@@ -4,7 +4,7 @@ neural-rendering resolution, 48+48 samples per ray).
 
     python bench.py --gpus 1 --steps K --warmup W                     # this repository (CUDA, libp3d.so)
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
-    python bench.py --impl reference ...          # the UNMODIFIED reference (baseline/_ref) on the host cores, same config
+    python bench.py --impl reference ...          # the UNMODIFIED reference (oracle/_ref) on the host cores, same config
     python bench.py --impl reference-cuda ...     # the UNMODIFIED reference on the GPU through its own JIT-built plugins
     python bench.py --workload {seg2cat_smoke,seg2cat_512,seg2face_512,edge2car_128}     # BASELINE.json configs 1-4
 
@@ -54,7 +54,7 @@ def workload_config(workload, B, world, extra=None):
 
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi sampling of SM clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi sampling of SM clocks / throttle reasons during the timed region."""
     FIELDS = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
               'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
               'clocks_event_reasons.sw_power_cap')
@@ -115,7 +115,8 @@ def measured_peaks():
                 return json.load(fh), 'measured (MEASURED_PEAKS.json)'
         except (OSError, ValueError):
             pass
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0}, 'fallback (B200_PROFILING.md)'
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 tensor rate
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'fallback (H100 SXM data sheet, 700 W)'
 
 
 # ---------------------------------------------------------------------------------------------
@@ -150,10 +151,10 @@ def cpu_port_state(batch):
 
 
 def run_reference_arm(args):
-    """`--impl reference`: the UNMODIFIED reference (baseline/_ref, byte-identical copy of /root/reference) on the host
+    """`--impl reference`: the UNMODIFIED reference (oracle/_ref, the byte-identical copy build() makes of a reference checkout) on the host
     cores -- `G.synthesis` of its own TriPlaneSemanticEntangleGenerator, custom ops on their `_ref` branch, fp32, all host
     threads, same workload / batch / seeds / inputs as the product arm. Steps are capped by a time budget so the run ends
-    within a few minutes. Falls back to the oracle port only if baseline/_ref is absent."""
+    within a few minutes. Falls back to the oracle port only if oracle/_ref is absent."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
         return
@@ -179,7 +180,7 @@ def run_reference_arm(args):
         cpu_port_step(state)
         dt = time.perf_counter() - t0
         value, ms_step, steps, warm, kind, stages = 1.0 / dt, 1000 * dt, 1, 1, 'port', None
-        sample = '1 image through oracle/p3d_oracle (baseline/_ref missing)'
+        sample = '1 image through oracle/p3d_oracle (oracle/_ref missing)'
     line = {
         'impl': 'reference', 'metric': metric_name(args.workload), 'value': value, 'unit': 'images/s', 'n_gpus': args.gpus,
         'steps': steps, 'warmup': warm, 'ms_per_step': ms_step, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
@@ -194,7 +195,7 @@ def run_reference_arm(args):
 
 
 def run_reference_cuda_arm(args):
-    """`--impl reference-cuda`: the reference's stock CUDA path on one B200 (BASELINE.md plan item 2, the ">= 5x" baseline):
+    """`--impl reference-cuda`: the reference's stock CUDA path on one GPU (BASELINE.md plan item 2, the ">= 5x" baseline):
     its plugins are JIT-built on first use by its own torch_utils/custom_ops.py:61, convolutions are cuDNN, SR runs in fp16 as
     shipped; a second measurement uses force_fp32. CUDA events, inputs resident."""
     rank = int(os.environ.get('RANK', '0'))
@@ -204,7 +205,7 @@ def run_reference_cuda_arm(args):
     import ref_harness as rh
     from pix2pix3d_b200 import configs
     if not rh.available():
-        print(json.dumps({'impl': 'reference-cuda', 'unavailable': 'baseline/_ref missing (run baseline/vendor_reference.py)'}), flush=True)
+        print(json.dumps({'impl': 'reference-cuda', 'unavailable': 'oracle/_ref missing (built by __graft_entry__.build() where a reference checkout exists)'}), flush=True)
         return
     if not torch.cuda.is_available():
         print(json.dumps({'impl': 'reference-cuda', 'unavailable': 'no CUDA device'}), flush=True)
@@ -335,19 +336,23 @@ def stock_cuda_leg(args, B, timeout_s=900):
     return {'unavailable': 'reference-cuda child printed no JSON line', 'rc': r.returncode, 'stderr_tail': r.stderr[-1500:]}
 
 
-def render_traffic(workload, B):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the fused render kernel, from the committed ncu --set full
-    summary (profiles/render_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep)."""
-    path = os.path.join(ROOT, 'profiles', 'render_traffic.json')
-    try:
-        with open(path) as fh:
-            t = json.load(fh)
-        for e in t['captures']:
-            if e['workload'] == workload and e['batch'] == B:
-                return e['dram_bytes_per_launch'], e.get('source')
-    except (OSError, ValueError, KeyError):
-        pass
-    return None, None
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out, path):
+    """Write every output tensor of one G.synthesis step as <path>/<name>.npy in float32. When the outputs together exceed
+    DUMP_BYTES, each array larger than its equal share is replaced by a fixed sample of that many elements (flat indices
+    drawn once from a seeded generator, sorted), so two builds of the project can be compared output for output."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: v.detach().float().cpu().numpy() for k, v in out.items() if hasattr(v, 'detach')}
+    total = sum(a.size * 4 for a in arrays.values())
+    share = DUMP_BYTES // 4 // max(1, len(arrays))
+    for name, a in sorted(arrays.items()):
+        if total > DUMP_BYTES and a.size > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=share, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, name + '.npy'), np.ascontiguousarray(a, dtype=np.float32))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -365,7 +370,15 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--force-fp32', action='store_true', help='run the SR stacks in fp32 (reference default is fp16)')
     ap.add_argument('--no-graph', action='store_true', help='launch every kernel from Python instead of replaying a CUDA graph')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the outputs of the last step as DIR/<name>.npy (float32, at most 64 MB; '
+                         'G.synthesis workloads of --impl ours only)')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
+    if args.dump_outputs and (args.workload == 'train_step' or args.impl != 'ours'):
+        ap.error('--dump-outputs writes the outputs of this package\'s G.synthesis: not available with --workload train_step '
+                 'or the reference arms')
     if args.workload == 'train_step':
         if args.impl == 'reference':
             raise SystemExit('--workload train_step has the arms `ours` and `reference-cuda` (a CPU train step takes minutes per image)')
@@ -410,6 +423,7 @@ def main():
     if args.force_fp32:
         syn_kw['force_fp32'] = True
 
+    torch.manual_seed(0)          # the renderer's stratified jitter and importance draws: same inputs on every run
     graphed = None
     if not args.no_graph:
         from pix2pix3d_b200.graphs import GraphedSynthesis
@@ -451,6 +465,8 @@ def main():
     e1.record()
     barrier()
     ms = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     launches = graphed.native_launches if graphed is not None else (_lib.launch_count - launches0) / args.steps
     kev = native.kernel_events
     native.kernel_events = None
@@ -529,15 +545,12 @@ def main():
     peaks, peak_src = measured_peaks()
     alg_bytes = configs.render_algorithmic_bytes(B, nrr * nrr, S)
     roofline = None
-    traffic, traffic_src = render_traffic(WORKLOAD, B)
     if render_ms:
         t_k = sum(render_ms) / len(render_ms) / 1000.0
         achieved = alg_bytes / t_k / 1e9
         roofline = {'kernel': 'render_fwd_tc_kernel' if native.render_impl in ('auto', 'tc') else 'render_fwd_kernel', 'bound': 'hbm', 'achieved': achieved, 'peak': peaks['hbm_gbs'], 'unit': 'GB/s',
                     'frac': achieved / peaks['hbm_gbs'],
-                    # dram__bytes_read + write per launch of this kernel at this workload, read from the committed ncu --set full
-                    # summary (profiles/render_traffic.json); null when no capture of this workload/batch exists
-                    'traffic': traffic, 'traffic_source': traffic_src, 'peak_source': peak_src,
+                    'peak_source': peak_src,
                     'kernel_ms': t_k * 1000, 'algorithmic_bytes': alg_bytes, 'share_of_step': t_k * 1000 / (ms / args.steps),
                     'rays_per_s': B * nrr * nrr / t_k}
 
@@ -564,7 +577,7 @@ def main():
             r = rh.time_synthesis(WORKLOAD, 'cpu', B, steps=2, warmup=2, budget_s=30)
             cpu_baseline = {'value': r['images_per_s'], 'unit': 'images/s', 'cores': r['threads'], 'kind': 'reference',
                             'sample': f"{r['steps']} steps x G.synthesis of {B} images through the unmodified reference on CPU "
-                                      f"(baseline/_ref, _ref ops, fp32, {r['threads']} torch threads = fastest of a sweep, "
+                                      f"(oracle/_ref, _ref ops, fp32, {r['threads']} torch threads = fastest of a sweep, "
                                       f"{os.cpu_count()} host cores) after {r['warmup']} warm-up steps, "
                                       f"{r['ms_per_step'] / 1000:.1f} s per step",
                             'stage_ms_per_step': r['stage_ms_per_step']}
@@ -574,7 +587,7 @@ def main():
             cpu_port_step(state)
             dt = time.perf_counter() - t0
             cpu_baseline = {'value': 1.0 / dt, 'unit': 'images/s', 'cores': os.cpu_count(), 'kind': 'port',
-                            'sample': f'1 image through oracle/p3d_oracle (baseline/_ref missing), {dt:.1f} s'}
+                            'sample': f'1 image through oracle/p3d_oracle (oracle/_ref missing), {dt:.1f} s'}
 
     # ---- reference stock CUDA path on this GPU (child process) ---------------------------------------
     stock_cuda, vs_stock = None, None
@@ -594,7 +607,7 @@ def main():
         'data': 'synthetic',
         'config': workload_config(WORKLOAD, B, world, {
                    'launch': 'CUDA graph replay of G.synthesis (pix2pix3d_b200.graphs.GraphedSynthesis)' if graphed is not None else 'eager',
-                   'l2_policy': 'no flush: per-step working set (planes 100 MB + SR activations > 2 GB) exceeds the 126 MB L2'}),
+                   'l2_policy': 'no flush: per-step working set (planes 100 MB + SR activations > 2 GB) exceeds the 50 MB L2'}),
         'rays_per_s': world * B * nrr * nrr * args.steps / (ms / 1000.0),
         'gpu_launches': launches,
         'e2e': {'value': e2e_value, 'unit': 'images/s', 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': d2h,

@@ -1,5 +1,5 @@
 /*
- * p3d.h -- C-ABI of libp3d.so, the sm_100a replacement for pix2pix3D's render + StyleGAN2-op hot path.
+ * p3d.h -- C-ABI of libp3d.so, the sm_90a replacement for pix2pix3D's render + StyleGAN2-op hot path.
  *
  * Every entry point takes plain device pointers, sizes and a CUDA stream; the caller owns all
  * memory (allocates outputs, keeps inputs alive until the stream reaches the call). Nothing is
@@ -139,7 +139,7 @@ int p3d_ray_limits_box(const float* rays_o, const float* rays_d, int64_t N, floa
  * -> fine sample+decode -> unify_samples (:157-167) -> final ray march, as one persistent kernel. */
 int p3d_render_fwd(const p3d_render_args_t* args, p3d_stream_t stream);
 
-/* Tensor-core variant of the same pipeline (decoder MLP on tcgen05 with fp16 hi/lo split operands and fp32 TMEM
+/* Tensor-core variant of the same pipeline (decoder MLP on wgmma with fp16 hi/lo split operands and fp32
  * accumulation; pix2pix3d_b200/csrc/render_tc.cu). Takes the decoder image of p3d_pack_decoder_tc. Returns
  * P3D_UNSUPPORTED when Sc or Sf is not a multiple of 8 (callers then use p3d_render_fwd). */
 #define P3D_DECODER_TC_PACKED_BYTES (65536 + 324 * 4)
@@ -153,7 +153,7 @@ int p3d_run_model(const float* planes_nhwc, const float* coords, const float* de
                   int B, int M, int H, int W, float coord_scale,
                   float* out_rgb, float* out_sigma, p3d_stream_t stream);
 
-/* The same query with the decoder MLP on tcgen05 (pix2pix3d_b200/csrc/query_tc.cu): the call behind
+/* The same query with the decoder MLP on wgmma (pix2pix3d_b200/csrc/query_tc.cu): the call behind
  * TriPlane*Generator.sample / sample_mixed (triplane_cond.py:1063-1074), e.g. the 512^3 sigma grid of
  * applications/extract_mesh.py:60-81. decoder_tc_packed is the image of p3d_pack_decoder_tc; plane_strides as in
  * p3d_render_args_t (NULL or all zero = dense [B,3,H,W,32]). out_rgb may be NULL: densities only (what extract_mesh
@@ -304,7 +304,7 @@ typedef struct {
     /* strided convolutions (conv2d_resample.py:108-111, the down=2 layers of DiscriminatorBlock / the label-map Encoder):
      * output pixel (y, x) reads input pixels (stride*y + dy, stride*x + dx); stride 0/1 = dense, 2 supported. */
     int32_t stride;
-    int32_t launch_flags;     /* A/B switches, results unchanged: bit 0 = never the persistent kernel, bit 1 = never CTA pairs */
+    int32_t launch_flags;     /* reserved: no kernel variant reads it (kept so the struct layout stays ABI 5) */
     /* resnet skip connection (networks_stylegan2.py:524-528): fp32 [B, oH, oW, Cout] (32-byte aligned, Cout % 8 == 0 for the
      * vector path) added after activation / gain / clamp; out_mode 0-2 with the identity output map. NULL = none. */
     const float* residual;
@@ -314,7 +314,7 @@ typedef struct {
      * consecutive samples. 0 = the single [oH*oW] image of noise_mode='const' shared by the batch. */
     int64_t noise_batch_stride;
     /* Fused 1x1 ToRGB of the NEXT layer (ABI 5; all zero = off): a launch whose single channel tile holds every output channel
-     * (Cout == Cout_padded <= 128, a multiple of 32; out_mode 0; 1:1 output map; persistent kernel) also evaluates, per pixel,
+     * (Cout == Cout_padded <= 128, a multiple of 32; out_mode 0; 1:1 output map; one phase) also evaluates, per pixel,
      *   rgb[c] = round16(clamp(dot(x_out[:], rgb_w[b][c][:]) * rgb_acc_scale + rgb_bias[c]))       c < rgb_cout <= 8
      * on the fp16-rounded outputs it has in registers, and writes rgb_out [B, rgb_cout, oH, oW] (fp32 NCHW) =
      * upsample2d(rgb_prev [B, oH/2, oW/2, rgb_cout] fp32 NHWC, rgb_filter) + rgb -- SynthesisBlock.forward's ToRGB + skip
@@ -330,7 +330,7 @@ typedef struct {
     float rgb_clamp, rgb_acc_scale;
 } p3d_conv_args_t;
 
-/* One implicit-GEMM convolution launch (tcgen05 + TMA): 3x3 / 1x1 convolutions and the four phases of a stride-2
+/* One implicit-GEMM convolution launch (wgmma + TMA): 3x3 / 1x1 convolutions and the four phases of a stride-2
  * transposed 3x3 convolution are all expressed through the tap list and the output map. */
 int p3d_conv_gemm(const p3d_conv_args_t* args, p3d_stream_t stream);
 

@@ -1,8 +1,8 @@
-"""Generate tests/golden/*.npz by running the REFERENCE implementation (imported read-only from /root/reference)
-on CPU with seeded inputs.
+"""Generate tests/golden/*.npz by running the REFERENCE implementation (a pix2pix3D checkout, imported read-only from
+$P3D_REFERENCE_ROOT) on CPU with seeded inputs.
 
-Runs only in the authoring container: the GPU box has no /root/reference, which is why the outputs are committed.
-    python oracle/make_golden.py            # writes tests/golden/{renderer,ops,synthesis}_*.npz and loss_ops.npz
+The tests never import the reference, which is why its outputs are committed.
+    P3D_REFERENCE_ROOT=/path/to/pix2pix3D python oracle/make_golden.py     # tests/golden/{renderer,ops,synthesis}_*.npz, loss_ops.npz
 
 The renderer's two random draws (stratified jitter, renderer.py:190; importance u, renderer.py:237) are captured
 by wrapping torch.rand_like / torch.rand while the reference runs, and stored so that every implementation can be
@@ -16,7 +16,7 @@ import sys
 import numpy as np
 import torch
 
-REF = '/root/reference'
+REF = os.environ.get('P3D_REFERENCE_ROOT', '')
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', 'tests', 'golden')
 
 
@@ -530,8 +530,50 @@ def golden_fullsize():
         print('fullsize', name, {k: tuple(v.shape) for k, v in out.items()}, os.path.getsize(os.path.join(OUT, f'{name}.npz')) // 1024, 'KiB')
 
 
+# tests/test_gpu_vs_reference.py: G.synthesis of the generator configurations behind BASELINE.json configs 1 and 3, inputs from
+# seed 7, fp32 on both sides; stored on a fixed grid (every 16th pixel of the 512^2 outputs, every 4th of the neural-rendering
+# outputs, odd offsets) so that the two fixtures stay small
+VSREF_CASES = {'vsref_seg2cat_512': dict(workload='seg2cat_512', B=2, input_seed=7),
+               'vsref_edge2car_128': dict(workload='edge2car_128', B=3, input_seed=7)}
+_SUB16 = (slice(None), slice(None), slice(3, None, 16), slice(5, None, 16))
+_SUB4 = (slice(None), slice(None), slice(1, None, 4), slice(2, None, 4))
+VSREF_SUB = {'image': _SUB16, 'semantic': _SUB16, 'image_raw': _SUB4, 'image_depth': _SUB4, 'semantic_raw': _SUB4}
+
+
+def golden_vs_reference():
+    import training.triplane_cond as ref_tc
+    repo = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..')
+    sys.path.append(repo)
+    from pix2pix3d_b200 import configs
+    for name, case in VSREF_CASES.items():
+        kw = configs.generator_kwargs(case['workload'])
+        kw['mapping_kwargs'] = dict(class_name='training.networks_stylegan2.MappingNetwork', num_layers=2)
+        torch.manual_seed(0)
+        G = ref_tc.TriPlaneSemanticEntangleGenerator(**kw).eval().requires_grad_(False)
+        gen = torch.Generator().manual_seed(1)
+        for pname, p in G.named_parameters():
+            if pname.endswith('noise_strength'):
+                p.copy_(torch.randn([], generator=gen) * 0.1)
+        w = configs.WORKLOADS[case['workload']]
+        rk = kw['rendering_kwargs']
+        nrr, Sc, Sf = w['nrr'], rk['depth_resolution'], rk['depth_resolution_importance']
+        ws, c, jitter, u = fullsize_inputs(case, G.backbone.num_ws, nrr, Sc, Sf)
+        it = iter([jitter, u])
+        o_like, o_rand = torch.rand_like, torch.rand
+        torch.rand_like, torch.rand = (lambda x, *a, **k: next(it)), (lambda *a, **k: next(it))
+        try:
+            with torch.no_grad():
+                out = G.synthesis(ws, c, noise_mode='const', neural_rendering_resolution=nrr, force_fp32=True)
+        finally:
+            torch.rand_like, torch.rand = o_like, o_rand
+        arrays = {'out_' + k: out[k][VSREF_SUB[k]].contiguous().numpy() for k in VSREF_SUB}
+        arrays['state_digest'] = np.frombuffer(state_digest(G).encode(), dtype=np.uint8)
+        np.savez_compressed(os.path.join(OUT, f'{name}.npz'), **arrays)
+        print('vs_reference', name, {k: tuple(v.shape) for k, v in arrays.items()}, os.path.getsize(os.path.join(OUT, f'{name}.npz')) // 1024, 'KiB')
+
+
 if __name__ == '__main__':
-    assert os.path.isdir(REF), 'the reference checkout is only available in the authoring container'
+    assert os.path.isdir(REF), 'set P3D_REFERENCE_ROOT to a checkout of the reference'
     sys.path.insert(0, REF)
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(os.cpu_count())
@@ -550,3 +592,5 @@ if __name__ == '__main__':
         golden_fullsize()
     if 'extra' in which:
         golden_extra()
+    if 'vs_reference' in which:
+        golden_vs_reference()

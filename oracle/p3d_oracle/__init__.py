@@ -6,7 +6,7 @@ cpu_baseline / --impl reference legs of bench.py -- never by pix2pix3d_b200 (the
 when its CUDA library is missing.
 
 Pinning: the reference ships no tests or golden vectors (SURVEY.md section 4). The oracle is pinned against the
-reference's own Python implementation, imported from /root/reference and run on CPU in the authoring container by
+reference's own Python implementation, imported from a reference checkout and run on CPU by
 oracle/make_golden.py; the resulting fixtures live in tests/golden/ and tests/test_oracle_golden.py checks the
 oracle against them. Dense-convolution arithmetic that the reference itself delegates to ATen
 (F.conv2d / F.conv_transpose2d, torch_utils/ops/conv2d_gradfix.py:40-45) is available both ways: ATen's CPU

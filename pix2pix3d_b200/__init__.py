@@ -1,4 +1,4 @@
-"""pix2pix3d_b200 -- sm_100a implementation of pix2pix3D's volumetric-rendering + StyleGAN2-op hot path.
+"""pix2pix3d_b200 -- sm_90a (H100) implementation of pix2pix3D's volumetric-rendering + StyleGAN2-op hot path.
 
 Layout
   csrc/            CUDA kernels and the C-ABI (include/p3d.h) -> libp3d.so (built by `pix2pix3d_b200.build`)

@@ -1,4 +1,4 @@
-"""Ahead-of-time build of libp3d.so (sm_100a only) with nvcc.
+"""Ahead-of-time build of libp3d.so (sm_90a only) with nvcc.
 
 Unlike the reference's JIT loader (torch_utils/custom_ops.py:61-157 in the reference repo) nothing is
 compiled at first call: `python -m pix2pix3d_b200.build` (or __graft_entry__.build()) produces
@@ -15,7 +15,7 @@ OUT = os.path.join(HERE, 'libp3d.so')
 STAMP = os.path.join(HERE, 'csrc', '.build_stamp')
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-O3', '-lineinfo', '-std=c++17',
     '-Xcompiler', '-fPIC', '-Xcompiler', '-O3',
     '--expt-relaxed-constexpr',
@@ -77,7 +77,7 @@ def build(force=False, verbose=False):
             fh.write(src_digest)
         with open(src[:-3] + '.ptxas.log', 'w') as fh:
             fh.write(out)
-    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', OUT] + objs
+    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', OUT] + objs
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -1,4 +1,4 @@
-// bias_act for sm_100a: y = clamp(act(x + b) * gain), plus the first/second-order gradient forms.
+// bias_act for sm_90a: y = clamp(act(x + b) * gain), plus the first/second-order gradient forms.
 // Replaces torch_utils/ops/bias_act.cu:27-151 + bias_act.cpp:36-94 of the reference.
 // Pure HBM streaming: 128-bit vector loads/stores, 64-bit indexing, grid = multiple of the SM count.
 #include "p3d_common.cuh"

@@ -1,8 +1,8 @@
-// Implicit-GEMM convolution on the 5th-generation tensor cores (tcgen05, sm_100a) for the modulated 3x3 / 1x1
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma, sm_90a) for the modulated 3x3 / 1x1
 // convolutions of the synthesis and super-resolution blocks (reference: training/networks_stylegan2.py:34-91,
 // torch_utils/ops/conv2d_resample.py:48-143, which bottom out in cuDNN).
 //
-//   D[128 pixels x BN channels] (TMEM, fp32) += A[128 x 64] (smem) * B[BN x 64]^T (smem), fp16 operands
+//   D[128 pixels x BN channels] (registers of two warpgroups, fp32) += A[128 x 64] (smem) * B[BN x 64]^T (smem), fp16 operands
 //
 // * Activations are NHWC fp16, so the im2col operand of one filter tap is a plain 4-D TMA box
 //   {64 channels, BW, BH, 1 image} shifted by the tap offset; out-of-bounds coordinates are zero-filled by the
@@ -10,24 +10,25 @@
 // * Weights are pre-modulated per sample (w * style * demod, fused_modconv semantics) and stored K-major
 //   [B][Cout][taps*Cin] fp16.
 // * fp32 layers (the tri-plane backbone) run as three fp16 passes over split operands, x = hi + lo,
-//   hi*hi + hi*lo + lo*hi, accumulated in the same fp32 TMEM tile (error ~2^-22, products are exact in fp32).
-// * Warp roles: warp 0 = TMA producer, warp 1 = TMEM owner + single-thread MMA issuer, warps 2-5 = epilogue
-//   (tcgen05.ld -> scale/noise/bias/activation/clamp -> NHWC store). mbarrier ring of kStages smem stages.
+//   hi*hi + hi*lo + lo*hi, accumulated in the same fp32 accumulators (error ~2^-22, products are exact in fp32).
+// * Warp roles: warp 8 = TMA producer, warps 0-7 = two consumer warpgroups (wgmma, then the epilogue:
+//   scale/noise/bias/activation/clamp -> NHWC store). mbarrier ring of smem stages.
 // * A launch may carry up to four PHASES (ConvPhase: tap subset, grid, output offset): the four parities of a stride-2
-//   transposed 3x3 convolution run as one launch whose tile order walks them heaviest first (p3d_conv_gemm_phases).
-// * The persistent kernel can also evaluate the NEXT layer's 1x1 ToRGB + skip on the outputs it holds (rgb_* arguments): the last
+//   transposed 3x3 convolution run as one launch (p3d_conv_gemm_phases).
+// * The kernel can also evaluate the NEXT layer's 1x1 ToRGB + skip on the outputs it holds (rgb_* arguments): the last
 //   super-resolution block then needs no ToRGB launch and never writes its activation tensor.
 #include <stdlib.h>
 #include <string.h>
 #include "p3d_common.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 #include "tmap.cuh"
 
 namespace p3d {
 
-constexpr int kBM = 128;        // pixels per tile (= TMEM lanes)
+constexpr int kBM = 128;        // pixels per tile (two warpgroups of 64 rows)
 constexpr int kBK = 64;         // fp16 elements per k-step (128-byte swizzle span)
 constexpr int kMaxGroups = 27;  // 9 taps x 3 precision passes
+constexpr int kMaxStages = 6;   // deepest smem ring
 
 // One output phase of a launch. An ordinary convolution has one; a stride-2 transposed convolution run as ONE launch has four
 // (tap subsets of the same weight tensor over the same input, each writing its own parity of the (2H+1) x (2W+1) grid).
@@ -48,7 +49,6 @@ struct ConvKernelArgs {
     int Cin;
     // tiling
     int BW, BH, BN, w_per_sample;
-    uint32_t idesc, tmem_cols;
     // epilogue
     int oH, oW, sy, sx;               // output tensor size and the stride of the output map (Y = y*sy + phase.oy)
     int Cout, y_cstride, y_coff;      // valid channels, channel stride of the output tensor, channel offset
@@ -83,17 +83,14 @@ __device__ __forceinline__ ConvPhase conv_phase_of(const ConvKernelArgs& a, int 
     return P;
 }
 
-// 256-bit global accesses (sm_100): one full 32-byte sector per lane
+// 32-byte global accesses (one full sector per lane) as two 16-byte vector instructions
 __device__ __forceinline__ void st_global_256(void* p, const uint32_t (&v)[8]) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-                 "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
+    asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
+    asm volatile("st.global.v4.b32 [%0+16], {%1, %2, %3, %4};" ::"l"(p), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
 }
 __device__ __forceinline__ void ld_global_256(const void* p, uint32_t (&v)[8]) {
-    asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "l"(p)
-                 : "memory");
+    asm volatile("ld.global.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(p) : "memory");
+    asm volatile("ld.global.v4.b32 {%0, %1, %2, %3}, [%4+16];" : "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "l"(p) : "memory");
 }
 
 // kAct: 0 linear, 1 leaky-relu with 0 <= alpha <= 1 (max form), 2 leaky-relu, any alpha (select form)
@@ -246,13 +243,15 @@ __device__ __forceinline__ void conv_store_chunk(const ConvKernelArgs& a, uint32
                     const int nvalid = min(32, a.Cout - ch0);
     #pragma unroll
                     for (int i = 0; i < 32; ++i) {
+                        if (xq && i >= nvalid) xq[i] = 0.f;
                         if (i < nvalid) {
                             float x = conv_epilogue_act<kAct, kClamp>(
                                 fmaf(__uint_as_float(v[i]), s_scale[c0 + i], s_bias[c0 + i]) + nz, alpha, post_gain, clampv);
                             if (a.residual) x += __ldg(a.residual + (((size_t)b * a.oH + Y) * a.oW + X) * a.Cout + ch0 + i);
                             if (out_mode <= 1) {
                                 const __half h = __float2half_rn(x);
-                                reinterpret_cast<__half*>(a.y)[off + i] = h;
+                                if (xq) xq[i] = __half2float(h);     // the fp16-rounded outputs, for the fused ToRGB of the next layer
+                                if (do_store) reinterpret_cast<__half*>(a.y)[off + i] = h;
                                 if (out_mode == 1) reinterpret_cast<__half*>(a.y_lo)[off + i] = __float2half_rn(x - __half2float(h));
                             } else {
                                 float* yf = reinterpret_cast<float*>(a.y) + off + i;
@@ -263,22 +262,31 @@ __device__ __forceinline__ void conv_store_chunk(const ConvKernelArgs& a, uint32
                 }
 }
 
-template <int kStages, int kAct, bool kClamp>
-__global__ void __launch_bounds__(192, 2) conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                           const __grid_constant__ CUtensorMap tmB,
-                                                           const ConvKernelArgs a) {
+// Warp roles: warps 0-7 = two consumer warpgroups (wgmma on tile rows 0-63 and 64-127, then the epilogue), warp 8 = TMA
+// producer. After the k-loop the accumulators are parked in the (then idle) stage ring as an fp32 [128 pixels][BN] tile so
+// that an epilogue thread owns one pixel and reads 32 consecutive channels, the form conv_store_chunk takes.
+constexpr int kConvThreads = 288;
+
+template <int kBN>
+__host__ __device__ constexpr int conv_stage_stride() { return (kBN > 32 ? kBN : 32) + 4; }   // floats per parked row
+
+template <int kAct, bool kClamp, int kBN>
+__global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                   const __grid_constant__ CUtensorMap tmB,
+                                                                   const ConvKernelArgs a, int n_stages) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [stages][A 16 KB][B BN*128 B] | barriers | tmem ptr | per-channel scale, bias
+    // carve: [stages][A 16 KB][B BN*128 B] | barriers | per-channel scale, bias | fused ToRGB weights [8][128]
     // round up inside the shared window (pointer arithmetic on smem_raw keeps the address space known to the compiler)
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-    const uint32_t a_bytes = (uint32_t)kBM * 128, b_bytes = (uint32_t)a.BN * 128;
+    const uint32_t a_bytes = (uint32_t)kBM * 128, b_bytes = (uint32_t)kBN * 128;
     const uint32_t stage_bytes = a_bytes + b_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * stage_bytes);
-    uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full_bar = empty_bar + kStages;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-    float* s_scale = reinterpret_cast<float*>(smem + kStages * stage_bytes + (((2 * kStages + 1) * 8 + 4 + 15) & ~15));
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + n_stages * stage_bytes);
+    uint64_t* empty_bar = full_bar + kMaxStages;
+    float* s_scale = reinterpret_cast<float*>(empty_bar + kMaxStages);
     float* s_bias = s_scale + 128;
+    float* s_rgbw = s_bias + 128;
+    float* s_acc = reinterpret_cast<float*>(smem);            // parked accumulators (after the k-loop)
+    constexpr int kSS = conv_stage_stride<kBN>();
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile_n = blockIdx.y;
@@ -286,27 +294,25 @@ __global__ void __launch_bounds__(192, 2) conv_gemm_kernel(const __grid_constant
     const int tile_m = (int)blockIdx.x - P.t0;
     const int b = blockIdx.z / a.splits, ksplit = blockIdx.z - b * a.splits;
     const int ty = tile_m / P.tiles_x, tx = tile_m % P.tiles_x;
-    const int n0 = tile_n * a.BN;
+    const int n0 = tile_n * kBN;
     const int all_k = P.ng * a.kc_steps;
     const int k_begin = (int)((long long)all_k * ksplit / a.splits), k_end = (int)((long long)all_k * (ksplit + 1) / a.splits);
     const int total_k = k_end - k_begin;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tc::tma_prefetch_desc(&tmA);
         tc::tma_prefetch_desc(&tmB);
-        for (int s = 0; s < kStages; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-        tc::mbar_init(tmem_full_bar, 1);
+        for (int s = 0; s < n_stages; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 8); }
         tc::fence_barrier_init();
     }
-    if (warp == 1) tc::tmem_alloc(tmem_ptr_smem, a.tmem_cols);
-    if (warp >= 2) {
+    if (warp < 8) {
         // per-channel epilogue constants: accumulator scale (1/weight scale x demodulation x gain) and bias x gain; channels
         // beyond Cout get zeros so the hot loop needs no channel predicate
-        const int i = threadIdx.x - 64;
-        if (i < a.BN) {
+        const int i = threadIdx.x;
+        if (i < 128) {
             const int ch = n0 + i;
             float sc = 0.f, bi = 0.f;
-            if (ch < a.Cout) {
+            if (i < kBN && ch < a.Cout) {
                 sc = a.acc_scale * a.pre_gain;
                 if (a.dscale) sc *= __ldg(a.dscale + (size_t)b * a.Cout + ch);
                 if (a.bias) bi = __ldg(a.bias + ch) * a.pre_gain;
@@ -314,13 +320,17 @@ __global__ void __launch_bounds__(192, 2) conv_gemm_kernel(const __grid_constant
             s_scale[i] = sc;
             s_bias[i] = bi;
         }
+        if (a.rgb_w) {
+            // modulated ToRGB weights of this tile's sample as fp32 [8][128] (rows beyond rgb_cout are zero)
+            for (int j = i; j < 8 * 128; j += 256) {
+                const int c = j >> 7, k = j & 127;
+                s_rgbw[j] = (c < a.rgb_cout && k < a.Cout) ? __half2float(__ldg(a.rgb_w + ((size_t)b * a.rgb_w_rows + c) * a.Cout + k)) : 0.f;
+            }
+        }
     }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===== TMA producer =====
         if (lane == 0) {
             int stage = 0; uint32_t phase = 0;
@@ -335,447 +345,142 @@ __global__ void __launch_bounds__(192, 2) conv_gemm_kernel(const __grid_constant
                 tc::mbar_expect_tx(&full_bar[stage], stage_bytes);
                 tc::tma_load_5d(sa, &tmA, &full_bar[stage], kc * kBK, x0, y0, b, a.a_plane[g]);
                 tc::tma_load_4d(sb, &tmB, &full_bar[stage], kb + kc * kBK, n0, a.w_per_sample ? b : 0, a.b_plane[g]);
-                if (++stage == kStages) { stage = 0; phase ^= 1; }
+                if (++stage == n_stages) { stage = 0; phase ^= 1; }
                 if (++kc == a.kc_steps) { kc = 0; ++g; }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (int k = 0; k < total_k; ++k) {
-                tc::mbar_wait(&full_bar[stage], phase);
-                tc::tc_fence_after();
-                const uint32_t sa = tc::smem_u32(smem + stage * stage_bytes);
-                const uint64_t da = tc::umma_desc_k128(sa), db = tc::umma_desc_k128(sa + a_bytes);
+        return;
+    }
+
+    // ===== consumers: warpgroup wg computes tile rows [64 wg, 64 wg + 64) x BN channels =====
+    const int wg = warp >> 2, wq = warp & 3;
+    float acc[kBN / 2];
 #pragma unroll
-                for (int j = 0; j < kBK / 16; ++j)   // 4 MMAs of K=16: advance 32 bytes inside the swizzle span
-                    tc::umma_f16(tmem_base, da + (uint64_t)(j * 2), db + (uint64_t)(j * 2), a.idesc, (k | j) != 0);
-                tc::umma_commit(&empty_bar[stage]);                 // frees the smem stage when these MMAs retire
-                if (k == total_k - 1) tc::umma_commit(tmem_full_bar);
-                if (++stage == kStages) { stage = 0; phase ^= 1; }
-            }
+    for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
+    {
+        int stage = 0; uint32_t phase = 0, prev = 0;
+        for (int k = 0; k < total_k; ++k) {
+            tc::mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = tc::smem_u32(smem + stage * stage_bytes);
+            const uint64_t da = tc::wgmma_desc_k128(sa + (uint32_t)wg * 64 * 128), db = tc::wgmma_desc_k128(sa + a_bytes);
+            tc::wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < kBK / 16; ++j) tc::wgmma_ss(acc, da + (uint64_t)(j * 2), db + (uint64_t)(j * 2));
+            tc::wgmma_commit();
+            tc::wgmma_wait<1>();                              // the MMAs of the previous k-step have retired
+            if (k > 0 && lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == n_stages) { stage = 0; phase ^= 1; }
         }
-    } else {
-        // ===== epilogue: warps 2..5 own TMEM lane quarters (warp % 4); thread = pixel, 32 channels per TMEM load =====
-        const int q = warp & 3;
-        const int m = q * 32 + lane;                    // tile row = TMEM lane
-        const int gy = ty * a.BH + m / a.BW, gx = tx * a.BW + m % a.BW;
-        const bool pix_ok = (gy < P.gH) && (gx < P.gW);
-        const int Y = gy * a.sy + P.oy, X = gx * a.sx + P.ox;
-        const size_t pix = ((size_t)b * a.oH + Y) * a.oW + X;
-        const float nz = (a.noise && pix_ok) ? __ldg(a.noise + (size_t)b * a.noise_bstride + (size_t)Y * a.oW + X) * a.pre_gain : 0.f;
-        const int out_mode = a.out_mode;
-        // vector path: every 32-channel chunk of this CTA is full and its stores are 32-byte aligned
-        const bool vec_ok = a.base_aligned && ((n0 + a.BN) <= a.Cout) && (a.BN % 32 == 0) &&
-                            (out_mode <= 1 ? ((a.y_cstride % 16) == 0 && ((a.y_coff + n0) % 16) == 0)
-                                           : ((a.y_cstride % 8) == 0 && ((a.y_coff + n0) % 8) == 0));
-        tc::mbar_wait(tmem_full_bar, 0);
-        tc::tc_fence_after();
-        for (int c0 = 0; c0 < a.BN; c0 += 32) {
-            uint32_t v[32];
-            tc::tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            tc::tmem_ld_wait();
-            if (!pix_ok) continue;
-            const int ch0 = n0 + c0;
-            if (a.partial) {
-                // split-K: raw accumulators of this k-range; conv_splitk_finish_kernel sums the ranges and applies the epilogue
-                float* pp = a.partial + P.p0 + ((((size_t)ksplit * (gridDim.z / a.splits) + b) * P.gH + gy) * P.gW + gx) * a.Cout_pad + ch0;
-                const int ncols = min(32, a.BN - c0);
+        tc::wgmma_wait<0>();
+        tc::wgmma_hold(acc);
+    }
+    // every consumer is past its last MMA and every TMA load has landed: the stage ring is free for the parked tile
+    tc::named_bar_sync(1, 256);
+    {
+        const int r0 = wg * 64 + wq * 16 + (lane >> 2), c = 2 * (lane & 3);
 #pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    if (8 * j < ncols) {
-                        const uint32_t o[8] = {v[8 * j], v[8 * j + 1], v[8 * j + 2], v[8 * j + 3], v[8 * j + 4], v[8 * j + 5], v[8 * j + 6], v[8 * j + 7]};
-                        st_global_256(pp + 8 * j, o);
+        for (int i = 0; i < kBN / 8; ++i)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<float2*>(s_acc + (r0 + 8 * h) * kSS + 8 * i + c) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+    }
+    tc::named_bar_sync(1, 256);
+
+    // ===== epilogue: thread = pixel (tile row m); two threads per pixel split the 32-channel chunks, except for the fused
+    // ToRGB, whose dot products need every channel of the pixel in one thread =====
+    const int m = threadIdx.x & 127, part = threadIdx.x >> 7;
+    if (a.rgb_w && part == 1) return;
+    const int gy = ty * a.BH + m / a.BW, gx = tx * a.BW + m % a.BW;
+    const bool pix_ok = (gy < P.gH) && (gx < P.gW);
+    if (!pix_ok) return;
+    const int Y = gy * a.sy + P.oy, X = gx * a.sx + P.ox;
+    const size_t pix = ((size_t)b * a.oH + Y) * a.oW + X;
+    const float nz = a.noise ? __ldg(a.noise + (size_t)b * a.noise_bstride + (size_t)Y * a.oW + X) * a.pre_gain : 0.f;
+    const int out_mode = a.out_mode;
+    // vector path for a 32-channel chunk: the chunk is full (checked per chunk below: the channel tile may extend past Cout)
+    // and its stores are 32-byte aligned (chunk offsets are multiples of 32 channels, so the tile's alignment decides)
+    const bool vec_aligned = a.base_aligned && (out_mode <= 1 ? ((a.y_cstride % 16) == 0 && ((a.y_coff + n0) % 16) == 0)
+                                                              : ((a.y_cstride % 8) == 0 && ((a.y_coff + n0) % 8) == 0));
+    const float* row = s_acc + m * kSS;
+    float dot[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) dot[c] = 0.f;
+    const int c_step = a.rgb_w ? 32 : 64;
+    for (int c0 = a.rgb_w ? 0 : 32 * part; c0 < kBN; c0 += c_step) {
+        uint32_t v[32];
+#pragma unroll
+        for (int i = 0; i < 32; i += 4) {
+            const float4 t = *reinterpret_cast<const float4*>(row + c0 + i);
+            v[i] = __float_as_uint(t.x); v[i + 1] = __float_as_uint(t.y); v[i + 2] = __float_as_uint(t.z); v[i + 3] = __float_as_uint(t.w);
+        }
+        const int ch0 = n0 + c0;
+        if (a.partial) {
+            // split-K: raw accumulators of this k-range; conv_splitk_finish_kernel sums the ranges and applies the epilogue
+            float* pp = a.partial + P.p0 + ((((size_t)ksplit * (gridDim.z / a.splits) + b) * P.gH + gy) * P.gW + gx) * a.Cout_pad + ch0;
+            const int ncols = min(32, kBN - c0);
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (8 * j < ncols && ch0 + 8 * j < a.Cout_pad) {
+                    const uint32_t o[8] = {v[8 * j], v[8 * j + 1], v[8 * j + 2], v[8 * j + 3], v[8 * j + 4], v[8 * j + 5], v[8 * j + 6], v[8 * j + 7]};
+                    st_global_256(pp + 8 * j, o);
+                }
+            continue;
+        }
+        if (ch0 >= a.Cout) continue;
+        const size_t off = pix * a.y_cstride + a.y_coff + ch0;
+        const bool vec_ok = vec_aligned && ch0 + 32 <= a.Cout;
+        if (a.rgb_w) {
+            // fused ToRGB of the next layer: dot products of this pixel's fp16-rounded outputs with the 1x1 weights
+            float xq[32];
+            conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, off, nz, vec_ok, b, Y, X, xq, a.rgb_skip_x == 0);
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+                if (c < a.rgb_cout) {
+                    const float4* wr = reinterpret_cast<const float4*>(s_rgbw + c * 128 + c0);
+                    float acc_c = dot[c];
+#pragma unroll
+                    for (int qd = 0; qd < 8; ++qd) {
+                        const float4 w4 = wr[qd];
+                        acc_c = fmaf(xq[4 * qd], w4.x, acc_c); acc_c = fmaf(xq[4 * qd + 1], w4.y, acc_c);
+                        acc_c = fmaf(xq[4 * qd + 2], w4.z, acc_c); acc_c = fmaf(xq[4 * qd + 3], w4.w, acc_c);
                     }
-                continue;
+                    dot[c] = acc_c;
+                }
             }
-            if (ch0 >= a.Cout) continue;
-            const size_t off = pix * a.y_cstride + a.y_coff + ch0;
+        } else {
             conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, off, nz, vec_ok, b, Y, X);
         }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(tmem_base, a.tmem_cols);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Persistent variant for launches with many tiles: one CTA per SM walks a static tile schedule. A tile is 256 pixels
-// (two stacked 128-row sub-tiles that share every B stage) x BN channels, so a k-step moves 32 KB + BN*128 B for twice the
-// FLOPs of the kernel above (the mainloop is bound by the per-SM L2 -> shared-memory ingest rate, ~50 B/clk). The four
-// 128-column accumulators are double-buffered in TMEM (2 tiles x 2 sub-tiles = 512 columns), so the epilogue of tile i
-// (warps 2-9, one warp per sub-tile and lane quarter) runs under the MMAs of tile i+1.
-// ---------------------------------------------------------------------------------------------
-constexpr int kPStages = 4;
-
-template <int kAct, bool kClamp>
-__global__ void __launch_bounds__(320, 1) conv_gemm_persist_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                    const __grid_constant__ CUtensorMap tmB,
-                                                                    const ConvKernelArgs a, int n_tiles, int tiles_n) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-    const uint32_t a_bytes = 2u * kBM * 128, b_bytes = (uint32_t)a.BN * 128;
-    const uint32_t stage_bytes = a_bytes + b_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kPStages * stage_bytes);
-    uint64_t* empty_bar = full_bar + kPStages;
-    uint64_t* tmem_full_bar = empty_bar + kPStages;      // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2]
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-    float* s_const = reinterpret_cast<float*>(smem + kPStages * stage_bytes + 128);     // [2 parities][scale 128 | bias 128]
-    float* s_rgbw = s_const + 512;                                                      // [2 parities][8][128] (fused ToRGB only)
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (warp == 0 && lane == 0) {
-        tc::tma_prefetch_desc(&tmA);
-        tc::tma_prefetch_desc(&tmB);
-        for (int s = 0; s < kPStages; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { tc::mbar_init(&tmem_full_bar[s], 1); tc::mbar_init(&tmem_empty_bar[s], 8); }
-        tc::fence_barrier_init();
-    }
-    if (warp == 1) tc::tmem_alloc(tmem_ptr_smem, 512);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const ConvPhase P = conv_phase_of(a, tile);
-                const int lt = tile - P.t0, tiles_m = P.tiles_x * P.tiles_y;
-                const int tm = lt % tiles_m, tn = (lt / tiles_m) % tiles_n, b = lt / (tiles_m * tiles_n);
-                const int ty = tm / P.tiles_x, tx = tm % P.tiles_x;
-                const int n0 = tn * a.BN;
-                const int total_k = P.ng * a.kc_steps;
-                int g = P.g0, kc = 0;
-                for (int k = 0; k < total_k; ++k) {
-                    const int x0 = tx * a.BW * a.stride + a.dx[g], y0 = ty * 2 * a.BH * a.stride + a.dy[g];
-                    const int kb = a.tap[g] * a.Cin;
-                    tc::mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t* sa = smem + stage * stage_bytes;
-                    tc::mbar_expect_tx(&full_bar[stage], stage_bytes);
-                    tc::tma_load_5d(sa, &tmA, &full_bar[stage], kc * kBK, x0, y0, b, a.a_plane[g]);
-                    tc::tma_load_4d(sa + a_bytes, &tmB, &full_bar[stage], kb + kc * kBK, n0, a.w_per_sample ? b : 0, a.b_plane[g]);
-                    if (++stage == kPStages) { stage = 0; phase ^= 1; }
-                    if (++kc == a.kc_steps) { kc = 0; ++g; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            int as = 0; uint32_t aphase = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int total_k = conv_phase_of(a, tile).ng * a.kc_steps;
-                tc::mbar_wait(&tmem_empty_bar[as], aphase ^ 1);        // the epilogue drained this accumulator pair
-                tc::tc_fence_after();
-                const uint32_t acc0 = tmem_base + (uint32_t)(as * 256);
-                for (int k = 0; k < total_k; ++k) {
-                    tc::mbar_wait(&full_bar[stage], phase);
-                    tc::tc_fence_after();
-                    const uint32_t sa = tc::smem_u32(smem + stage * stage_bytes);
-                    const uint64_t da = tc::umma_desc_k128(sa), db = tc::umma_desc_k128(sa + a_bytes);
+    if (a.rgb_w) {
+        // out = upsample2d(prev)[b, Y, X, :] + round16(clamp(dot * scale + bias)), written NCHW (lanes = consecutive X)
+        const int ph = a.oH >> 1, pw = a.oW >> 1, C = a.rgb_cout;
+        const int iy = Y >> 1, py = Y & 1, ix = X >> 1, px = X & 1;
+        float w4[2][2];
+        const float* pp[2][2];
 #pragma unroll
-                    for (int mt = 0; mt < 2; ++mt) {
-                        const uint64_t dam = da + (uint64_t)(mt * (kBM * 128 >> 4));
+        for (int aa = 0; aa < 2; ++aa)
 #pragma unroll
-                        for (int j = 0; j < kBK / 16; ++j)
-                            tc::umma_f16(acc0 + (uint32_t)(mt * 128), dam + (uint64_t)(j * 2), db + (uint64_t)(j * 2), a.idesc, (k | j) != 0);
-                    }
-                    tc::umma_commit(&empty_bar[stage]);
-                    if (k == total_k - 1) tc::umma_commit(&tmem_full_bar[as]);
-                    if (++stage == kPStages) { stage = 0; phase ^= 1; }
-                }
-                if (++as == 2) { as = 0; aphase ^= 1; }
+            for (int cc = 0; cc < 2; ++cc) {
+                const int ry = iy - 1 + py + aa, rx = ix - 1 + px + cc;
+                const bool ok = ry >= 0 && ry < ph && rx >= 0 && rx < pw;
+                w4[aa][cc] = ok ? __ldg(a.rgb_f + (3 - (py + 2 * aa)) * 4 + (3 - (px + 2 * cc))) * 4.f : 0.f;
+                pp[aa][cc] = a.rgb_prev + (((size_t)b * ph + (ok ? ry : 0)) * pw + (ok ? rx : 0)) * C;
             }
-        }
-    } else {
-        // ===== epilogue: warps 2..9; sub-tile = (warp - 2) / 4, TMEM lane quarter = warp % 4 =====
-        const int e = warp - 2, mt = e >> 2, q = warp & 3;
-        const int m = q * 32 + lane;                    // row inside the 128-row sub-tile = TMEM lane
-        const int et = threadIdx.x - 64;                // 0..255 among the epilogue threads
-        int as = 0; uint32_t aphase = 0;
-        int parity = 0;
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const ConvPhase P = conv_phase_of(a, tile);
-            const int lt = tile - P.t0, tiles_m = P.tiles_x * P.tiles_y;
-            const int tm = lt % tiles_m, tn = (lt / tiles_m) % tiles_n, b = lt / (tiles_m * tiles_n);
-            const int ty = tm / P.tiles_x, tx = tm % P.tiles_x;
-            const int n0 = tn * a.BN;
-            float* s_scale = s_const + parity * 256;
-            float* s_bias = s_scale + 128;
-            if (et < a.BN) {
-                const int ch = n0 + et;
-                float sc = 0.f, bi = 0.f;
-                if (ch < a.Cout) {
-                    sc = a.acc_scale * a.pre_gain;
-                    if (a.dscale) sc *= __ldg(a.dscale + (size_t)b * a.Cout + ch);
-                    if (a.bias) bi = __ldg(a.bias + ch) * a.pre_gain;
-                }
-                s_scale[et] = sc;
-                s_bias[et] = bi;
-            }
-            float* s_rw = s_rgbw + parity * 1024;
-            if (a.rgb_w) {
-                // modulated ToRGB weights of this tile's sample as fp32 [8][128] (rows beyond rgb_cout are zero)
-                for (int i = et; i < 8 * 128; i += 256) {
-                    const int c = i >> 7, k = i & 127;
-                    s_rw[i] = (c < a.rgb_cout && k < a.Cout)
-                                  ? __half2float(__ldg(a.rgb_w + ((size_t)b * a.rgb_w_rows + c) * a.Cout + k)) : 0.f;
-                }
-            }
-            tc::named_bar_sync(1, 256);                 // constants of this tile visible to all epilogue warps
-            const int gy = (ty * 2 + mt) * a.BH + m / a.BW, gx = tx * a.BW + m % a.BW;
-            const bool pix_ok = (gy < P.gH) && (gx < P.gW);
-            const int Y = gy * a.sy + P.oy, X = gx * a.sx + P.ox;
-            const size_t pix = ((size_t)b * a.oH + Y) * a.oW + X;
-            const float nz = (a.noise && pix_ok) ? __ldg(a.noise + (size_t)b * a.noise_bstride + (size_t)Y * a.oW + X) * a.pre_gain : 0.f;
-            const bool vec_ok = a.base_aligned && ((n0 + a.BN) <= a.Cout) && (a.BN % 32 == 0) &&
-                                (a.out_mode <= 1 ? ((a.y_cstride % 16) == 0 && ((a.y_coff + n0) % 16) == 0)
-                                                 : ((a.y_cstride % 8) == 0 && ((a.y_coff + n0) % 8) == 0));
-            tc::mbar_wait(&tmem_full_bar[as], aphase);
-            tc::tc_fence_after();
-            const uint32_t acc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * 256 + mt * 128);
-            float dot[8];
 #pragma unroll
-            for (int c = 0; c < 8; ++c) dot[c] = 0.f;
-            for (int c0 = 0; c0 < a.BN; c0 += 32) {
-                uint32_t v[32];
-                tc::tmem_ld_32x32(acc + (uint32_t)c0, v);
-                tc::tmem_ld_wait();
-                const int ch0 = n0 + c0;
-                if (!pix_ok || ch0 >= a.Cout) continue;
-                if (a.rgb_w) {
-                    // fused ToRGB of the next layer: dot products of this pixel's fp16-rounded outputs with the 1x1 weights
-                    float xq[32];
-                    conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, pix * a.y_cstride + a.y_coff + ch0, nz, vec_ok, b, Y, X,
-                                                   xq, a.rgb_skip_x == 0);
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        if (c < a.rgb_cout) {
-                            const float4* wr = reinterpret_cast<const float4*>(s_rw + c * 128 + c0);
-                            float acc_c = dot[c];
-#pragma unroll
-                            for (int qd = 0; qd < 8; ++qd) {
-                                const float4 w4 = wr[qd];
-                                acc_c = fmaf(xq[4 * qd], w4.x, acc_c); acc_c = fmaf(xq[4 * qd + 1], w4.y, acc_c);
-                                acc_c = fmaf(xq[4 * qd + 2], w4.z, acc_c); acc_c = fmaf(xq[4 * qd + 3], w4.w, acc_c);
-                            }
-                            dot[c] = acc_c;
-                        }
-                    }
-                } else {
-                    conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, pix * a.y_cstride + a.y_coff + ch0, nz, vec_ok, b, Y, X);
-                }
-            }
-            tc::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(&tmem_empty_bar[as]);      // 8 warps -> accumulator pair free for the MMA warp
-            if (a.rgb_w && pix_ok) {
-                // out = upsample2d(prev)[b, Y, X, :] + round16(clamp(dot * scale + bias)), written NCHW (lanes = consecutive X)
-                const int ph = a.oH >> 1, pw = a.oW >> 1, C = a.rgb_cout;
-                const int iy = Y >> 1, py = Y & 1, ix = X >> 1, px = X & 1;
-                float w4[2][2];
-                const float* pp[2][2];
+        for (int c = 0; c < 8; ++c) {
+            if (c < C) {
+                float u = 0.f;
 #pragma unroll
                 for (int aa = 0; aa < 2; ++aa)
 #pragma unroll
-                    for (int cc = 0; cc < 2; ++cc) {
-                        const int ry = iy - 1 + py + aa, rx = ix - 1 + px + cc;
-                        const bool ok = ry >= 0 && ry < ph && rx >= 0 && rx < pw;
-                        w4[aa][cc] = ok ? __ldg(a.rgb_f + (3 - (py + 2 * aa)) * 4 + (3 - (px + 2 * cc))) * 4.f : 0.f;
-                        pp[aa][cc] = a.rgb_prev + (((size_t)b * ph + (ok ? ry : 0)) * pw + (ok ? rx : 0)) * C;
-                    }
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    if (c < C) {
-                        float u = 0.f;
-#pragma unroll
-                        for (int aa = 0; aa < 2; ++aa)
-#pragma unroll
-                            for (int cc = 0; cc < 2; ++cc) u = fmaf(w4[aa][cc], __ldg(pp[aa][cc] + c), u);
-                        float x = fmaf(dot[c], a.rgb_acc_scale, a.rgb_bias ? __ldg(a.rgb_bias + c) : 0.f);
-                        if (a.rgb_clamp >= 0.f) x = fminf(fmaxf(x, -a.rgb_clamp), a.rgb_clamp);
-                        x = __half2float(__float2half_rn(x));
-                        a.rgb_out[(((size_t)b * C + c) * a.oH + Y) * a.oW + X] = u + x;
-                    }
-                }
-            }
-            if (++as == 2) { as = 0; aphase ^= 1; }
-            parity ^= 1;
-        }
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(tmem_base, 512);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2) for layers with >= 256 output channels: the two CTAs of a cluster sit on the two SMs of a
-// TPC and issue ONE M=256 x N=256 MMA per k-step. Each CTA stages its own 128 pixel rows of A and HALF of the weight
-// tile (128 of the 256 channel rows), so a k-step costs 32 KB per SM for 4.2 MFLOP per SM (131 FLOP/B, against 87 for
-// the single-CTA persistent kernel) -- the quantity that bounds these kernels is bytes into each SM per FLOP.
-// Persistent over a static schedule of (256-pixel, 256-channel) tiles; accumulators double-buffered (2 x 256 TMEM columns
-// per CTA). Leader (cluster rank 0): counts both CTAs' TMA bytes on its `full` barriers and issues the MMAs; completion is
-// multicast to both CTAs' `empty` / `tmem_full` barriers; both CTAs' epilogue warps arrive on the leader's `tmem_empty`.
-// ---------------------------------------------------------------------------------------------
-constexpr int kQStages = 6;
-
-template <int kAct, bool kClamp>
-__global__ void __launch_bounds__(320, 1) conv_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                 const __grid_constant__ CUtensorMap tmB,
-                                                                 const ConvKernelArgs a, int n_tiles, int tiles_n) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-    constexpr uint32_t a_bytes = kBM * 128, b_bytes = 128 * 128, stage_bytes = a_bytes + b_bytes;   // per CTA
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kQStages * stage_bytes);
-    uint64_t* empty_bar = full_bar + kQStages;
-    uint64_t* tmem_full_bar = empty_bar + kQStages;      // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2] (the leader's are used)
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-    float* s_const = reinterpret_cast<float*>(smem + kQStages * stage_bytes + 256);     // [2 parities][scale 256 | bias 256]
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = tc::cluster_ctarank();
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-
-    if (warp == 0 && lane == 0) {
-        tc::tma_prefetch_desc(&tmA);
-        tc::tma_prefetch_desc(&tmB);
-        for (int s = 0; s < kQStages; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { tc::mbar_init(&tmem_full_bar[s], 1); tc::mbar_init(&tmem_empty_bar[s], 16); }
-        tc::fence_barrier_init();
-    }
-    if (warp == 1) tc::tmem_alloc_pair(tmem_ptr_smem, 512);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::cluster_sync_all();                               // both CTAs' barriers exist before any remote arrive / complete_tx
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-
-    if (warp == 0) {
-        // ===== TMA producer (both CTAs): own A rows, own half of B; bytes counted on the leader's barrier =====
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (int tile = pair; tile < n_tiles; tile += n_pairs) {
-                const ConvPhase P = conv_phase_of(a, tile);
-                const int lt = tile - P.t0, tiles_m = P.tiles_x * P.tiles_y;
-                const int tm = lt % tiles_m, tn = (lt / tiles_m) % tiles_n, b = lt / (tiles_m * tiles_n);
-                const int ty = tm / P.tiles_x, tx = tm % P.tiles_x;
-                const int n0 = tn * 256 + (int)rank * 128;
-                const int total_k = P.ng * a.kc_steps;
-                int g = P.g0, kc = 0;
-                for (int k = 0; k < total_k; ++k) {
-                    const int x0 = tx * a.BW * a.stride + a.dx[g], y0 = (ty * 2 + (int)rank) * a.BH * a.stride + a.dy[g];
-                    const int kb = a.tap[g] * a.Cin;
-                    tc::mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t* sa = smem + stage * stage_bytes;
-                    const uint32_t lead_full = tc::mapa_u32(tc::smem_u32(&full_bar[stage]), 0);
-                    if (rank == 0) tc::mbar_expect_tx(&full_bar[stage], 2 * stage_bytes);
-                    tc::tma_load_5d_pair(sa, &tmA, lead_full, kc * kBK, x0, y0, b, a.a_plane[g]);
-                    tc::tma_load_4d_pair(sa + a_bytes, &tmB, lead_full, kb + kc * kBK, n0, a.w_per_sample ? b : 0, a.b_plane[g]);
-                    if (++stage == kQStages) { stage = 0; phase ^= 1; }
-                    if (++kc == a.kc_steps) { kc = 0; ++g; }
-                }
+                    for (int cc = 0; cc < 2; ++cc) u = fmaf(w4[aa][cc], __ldg(pp[aa][cc] + c), u);
+                float x = fmaf(dot[c], a.rgb_acc_scale, a.rgb_bias ? __ldg(a.rgb_bias + c) : 0.f);
+                if (a.rgb_clamp >= 0.f) x = fminf(fmaxf(x, -a.rgb_clamp), a.rgb_clamp);
+                x = __half2float(__float2half_rn(x));
+                a.rgb_out[(((size_t)b * C + c) * a.oH + Y) * a.oW + X] = u + x;
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: one thread of the leader CTA =====
-        if (rank == 0 && lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            int as = 0; uint32_t aphase = 0;
-            for (int tile = pair; tile < n_tiles; tile += n_pairs) {
-                const int total_k = conv_phase_of(a, tile).ng * a.kc_steps;
-                tc::mbar_wait(&tmem_empty_bar[as], aphase ^ 1);        // both CTAs' epilogues drained this accumulator
-                tc::tc_fence_after();
-                const uint32_t acc = tmem_base + (uint32_t)(as * 256);
-                for (int k = 0; k < total_k; ++k) {
-                    tc::mbar_wait(&full_bar[stage], phase);
-                    tc::tc_fence_after();
-                    const uint32_t sa = tc::smem_u32(smem + stage * stage_bytes);
-                    const uint64_t da = tc::umma_desc_k128(sa), db = tc::umma_desc_k128(sa + a_bytes);
-#pragma unroll
-                    for (int j = 0; j < kBK / 16; ++j)
-                        tc::umma_f16_pair(acc, da + (uint64_t)(j * 2), db + (uint64_t)(j * 2), a.idesc, (k | j) != 0);
-                    tc::umma_commit_pair(&empty_bar[stage], 3);        // stage free in both CTAs
-                    if (k == total_k - 1) tc::umma_commit_pair(&tmem_full_bar[as], 3);
-                    if (++stage == kQStages) { stage = 0; phase ^= 1; }
-                }
-                if (++as == 2) { as = 0; aphase ^= 1; }
-            }
-        }
-    } else {
-        // ===== epilogue (both CTAs): warps 2..9; column half = (warp - 2) / 4, TMEM lane quarter = warp % 4 =====
-        const int e = warp - 2, hsel = e >> 2, q = warp & 3;
-        const int m = q * 32 + lane;
-        const int et = threadIdx.x - 64;                // 0..255
-        const uint32_t lead_empty0 = tc::mapa_u32(tc::smem_u32(&tmem_empty_bar[0]), 0);
-        const uint32_t lead_empty1 = tc::mapa_u32(tc::smem_u32(&tmem_empty_bar[1]), 0);
-        int as = 0; uint32_t aphase = 0;
-        int parity = 0;
-        for (int tile = pair; tile < n_tiles; tile += n_pairs) {
-            const ConvPhase P = conv_phase_of(a, tile);
-            const int lt = tile - P.t0, tiles_m = P.tiles_x * P.tiles_y;
-            const int tm = lt % tiles_m, tn = (lt / tiles_m) % tiles_n, b = lt / (tiles_m * tiles_n);
-            const int ty = tm / P.tiles_x, tx = tm % P.tiles_x;
-            const int n0 = tn * 256;
-            float* s_scale = s_const + parity * 512;
-            float* s_bias = s_scale + 256;
-            {
-                const int ch = n0 + et;
-                float sc = 0.f, bi = 0.f;
-                if (ch < a.Cout) {
-                    sc = a.acc_scale * a.pre_gain;
-                    if (a.dscale) sc *= __ldg(a.dscale + (size_t)b * a.Cout + ch);
-                    if (a.bias) bi = __ldg(a.bias + ch) * a.pre_gain;
-                }
-                s_scale[et] = sc;
-                s_bias[et] = bi;
-            }
-            tc::named_bar_sync(1, 256);
-            const int gy = (ty * 2 + (int)rank) * a.BH + m / a.BW, gx = tx * a.BW + m % a.BW;
-            const bool pix_ok = (gy < P.gH) && (gx < P.gW);
-            const int Y = gy * a.sy + P.oy, X = gx * a.sx + P.ox;
-            const size_t pix = ((size_t)b * a.oH + Y) * a.oW + X;
-            const float nz = (a.noise && pix_ok) ? __ldg(a.noise + (size_t)b * a.noise_bstride + (size_t)Y * a.oW + X) * a.pre_gain : 0.f;
-            const bool vec_ok = a.base_aligned && ((n0 + 256) <= a.Cout) &&
-                                (a.out_mode <= 1 ? ((a.y_cstride % 16) == 0 && ((a.y_coff + n0) % 16) == 0)
-                                                 : ((a.y_cstride % 8) == 0 && ((a.y_coff + n0) % 8) == 0));
-            tc::mbar_wait(&tmem_full_bar[as], aphase);
-            tc::tc_fence_after();
-            const uint32_t acc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * 256 + hsel * 128);
-            for (int c0 = 0; c0 < 128; c0 += 32) {
-                uint32_t v[32];
-                tc::tmem_ld_32x32(acc + (uint32_t)c0, v);
-                tc::tmem_ld_wait();
-                const int cc = hsel * 128 + c0, ch0 = n0 + cc;
-                if (!pix_ok || ch0 >= a.Cout) continue;
-                conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, cc, ch0, pix * a.y_cstride + a.y_coff + ch0, nz, vec_ok, b, Y, X);
-            }
-            tc::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive_cluster(as == 0 ? lead_empty0 : lead_empty1);
-            if (++as == 2) { as = 0; aphase ^= 1; }
-            parity ^= 1;
-        }
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::cluster_sync_all();                               // the peer may still be reading this CTA's smem / signalling its barriers
-    if (warp == 1) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc_pair(tmem_base, 512);
     }
 }
 
@@ -857,7 +562,7 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     if (p->Cout_padded % 16 != 0 || p->Cout_padded < p->Cout) return P3D_BAD_ARG;
     if (p->B <= 0) return P3D_BAD_ARG;
     const int passes = p->split ? 3 : 1;
-    int taps_total = 0, taps_max = 0, gH_max = 0, gW_max = 0;
+    int taps_total = 0, gH_max = 0, gW_max = 0;
     for (int q = 0; q < n_phases; ++q) {
         const p3d_conv_args_t* r = phases + q;
         if (r->n_taps < 1 || r->n_taps > 9 || r->gH <= 0 || r->gW <= 0) return q == 0 ? P3D_UNSUPPORTED : P3D_BAD_ARG;
@@ -871,47 +576,27 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
                       r->noise_batch_stride != p->noise_batch_stride || r->rgb_w || p->rgb_w))
             return P3D_BAD_ARG;
         taps_total += r->n_taps;
-        if (r->n_taps > taps_max) taps_max = r->n_taps;
         if (r->gH > gH_max) gH_max = r->gH;
         if (r->gW > gW_max) gW_max = r->gW;
     }
     if (taps_total * passes > kMaxGroups) return P3D_UNSUPPORTED;
 
-    const int BN = p->Cout_padded > 128 ? 128 : p->Cout_padded;
+    // channel tile = the wgmma N: 32, 64 or 128 (channels past Cout_padded are zero-filled by the TMA and never stored)
+    const int BN = p->Cout_padded > 64 ? 128 : p->Cout_padded > 32 ? 64 : 32;
     // spatial tile BW x BH = 128 pixels: the power-of-two split with the least padded area (ties -> wider rows), summed over
-    // the phases (they share the TMA box); `rows` = sub-tiles stacked in y per CTA tile (2 for the persistent kernels)
+    // the phases (they share the TMA box)
     const int stride = p->stride > 1 ? p->stride : 1;
     if (stride > 2) return P3D_UNSUPPORTED;
-    auto pick_bw = [&](int rows, long* area_out) {
-        int bw_best = 1;
+    int BW = 1;
+    {
         long best = -1;
         for (int bw = 1; bw <= 64; bw *= 2) {
-            int bh = kBM / bw * rows;
+            const int bh = kBM / bw;
             if (bw * stride > 256 || bh * stride > 256) continue;      // TMA box extent (in input pixels) <= 256
             long area = 0;
             for (int q = 0; q < n_phases; ++q) area += (long)ceil_div(phases[q].gW, bw) * bw * ceil_div(phases[q].gH, bh) * bh;
-            if (best < 0 || area <= best) { best = area; bw_best = bw; }
+            if (best < 0 || area <= best) { best = area; BW = bw; }
         }
-        if (area_out) *area_out = best;
-        return bw_best;
-    };
-    // persistent 256-pixel tiles when there is at least one tile per SM (launch_flags bit 0 disables, for A/B runs)
-    bool persist = false, pair = false;
-    int BW = pick_bw(1, nullptr);
-    {
-        const int env = (p->launch_flags & 1) ? 0 : 1;
-        long area2 = 0;
-        const int bw2 = pick_bw(2, &area2);
-        const long tiles2 = area2 / 256 * ceil_div(p->Cout_padded, BN) * p->B;
-        if (env && tiles2 >= sm_count()) { persist = true; BW = bw2; }
-        // CTA pairs (cta_group::2) for >= 256 output channels: one 256-pixel x 256-channel tile per pair
-        // (launch_flags bit 1 keeps the single-CTA persistent kernel, for A/B runs)
-        const int env_pair = (p->launch_flags & 2) ? 0 : 1;
-        const long tiles_pair = area2 / 256 * (p->Cout_padded / 256) * p->B;
-        // (launches with a handful of k-steps per tile -- the 1- and 2-tap phases of a narrow transposed convolution -- are
-        //  prologue/epilogue-bound and measured slightly slower on pairs; a merged launch is judged by its heaviest phase)
-        const int k_steps = passes * taps_max * (p->C / kBK);
-        if (persist && env_pair && p->Cout_padded % 256 == 0 && tiles_pair * 2 >= sm_count() && k_steps >= 8) pair = true;
     }
     const int BH = kBM / BW;
     const int K = p->n_kblocks * p->C;
@@ -924,7 +609,7 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
                            (uint64_t)p->B * p->H * p->W * p->C * 2};
         // a strided convolution samples every `stride`-th input pixel: the TMA walks the box with that element stride
         // (box extents are then given in input pixels: N loaded pixels need an extent of N * stride)
-        uint32_t box[5] = {(uint32_t)kBK, (uint32_t)(BW * stride), (uint32_t)(((persist && !pair) ? 2 * BH : BH) * stride), 1, 1};
+        uint32_t box[5] = {(uint32_t)kBK, (uint32_t)(BW * stride), (uint32_t)(BH * stride), 1, 1};
         uint32_t es[5] = {1, (uint32_t)stride, (uint32_t)stride, 1, 1};
         int rc = make_tmap_f16_sw128(&tmA, p->x, 5, dims, str, box, es);
         if (rc != P3D_OK) return rc;
@@ -932,7 +617,7 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     {
         uint64_t dims[4] = {(uint64_t)K, (uint64_t)p->Cout_padded, (uint64_t)p->Bw, (uint64_t)p->w_planes};
         uint64_t str[3] = {(uint64_t)K * 2, (uint64_t)p->Cout_padded * K * 2, (uint64_t)p->Bw * p->Cout_padded * K * 2};
-        uint32_t box[4] = {(uint32_t)kBK, (uint32_t)(pair ? 128 : BN), 1, 1};     // a pair CTA stages half of a 256-channel tile
+        uint32_t box[4] = {(uint32_t)kBK, (uint32_t)BN, 1, 1};
         int rc = make_tmap_f16_sw128(&tmB, p->w, 4, dims, str, box);
         if (rc != P3D_OK) return rc;
     }
@@ -940,7 +625,6 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     ConvKernelArgs a;
     memset(&a, 0, sizeof(a));
     static const int pa[3] = {0, 0, 1}, pb[3] = {0, 1, 0};     // hi*hi, hi*lo, lo*hi
-    const int tiles_n = pair ? p->Cout_padded / 256 : ceil_div(p->Cout_padded, BN);
     int g = 0, tiles_m_total = 0, max_total_k = 0, min_total_k = 1 << 30;
     a.n_phases = n_phases;
     a.kc_steps = p->C / kBK;
@@ -956,9 +640,8 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
             }
         P.ng = g - P.g0;
         P.gH = r->gH; P.gW = r->gW; P.oy = r->oy; P.ox = r->ox;
-        P.tiles_x = ceil_div(r->gW, BW); P.tiles_y = ceil_div(r->gH, persist ? 2 * BH : BH);
-        // tile order: spatial tiles for the grid kernel (blockIdx.x), whole (spatial, channel, sample) tiles for the persistent ones
-        P.t0 = persist ? tiles_m_total * tiles_n * p->B : tiles_m_total;
+        P.tiles_x = ceil_div(r->gW, BW); P.tiles_y = ceil_div(r->gH, BH);
+        P.t0 = tiles_m_total;                                   // spatial tiles of the phase: blockIdx.x range
         tiles_m_total += P.tiles_x * P.tiles_y;
         const int tk = P.ng * a.kc_steps;
         if (tk > max_total_k) max_total_k = tk;
@@ -967,8 +650,6 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     a.Cin = p->C;
     a.BW = BW; a.BH = BH;
     a.BN = BN; a.w_per_sample = p->Bw > 1 ? 1 : 0;
-    a.idesc = tc::umma_idesc_f16(kBM, BN, 0);
-    a.tmem_cols = BN <= 32 ? 32u : BN <= 64 ? 64u : 128u;
     a.oH = p->oH; a.oW = p->oW; a.sy = p->sy; a.sx = p->sx;
     a.Cout = p->Cout; a.y_cstride = p->y_cstride; a.y_coff = p->y_coff;
     a.y = p->y; a.y_lo = p->y_lo; a.out_mode = p->out_mode;
@@ -979,9 +660,9 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     a.up_prev = p->up_prev; a.up_f = p->up_filter; a.round16 = p->round16; a.out_nchw = p->out_nchw;
     a.stride = stride; a.residual = p->residual;
     if (p->rgb_w) {
-        // fused ToRGB of the next layer: one channel tile holding every output channel, fp16 output, 1:1 output map, persistent
-        // single-CTA kernel (its epilogue thread sees all channels of its pixel)
-        if (n_phases != 1 || !persist || pair || p->up_prev || p->residual || p->out_mode != 0 || p->Cout != p->Cout_padded ||
+        // fused ToRGB of the next layer: one channel tile holding every output channel, fp16 output, 1:1 output map (the
+        // epilogue thread of a pixel sees all of its channels)
+        if (n_phases != 1 || p->up_prev || p->residual || p->out_mode != 0 || p->Cout != p->Cout_padded ||
             p->Cout > 128 || p->Cout % 32 != 0 || p->sy != 1 || p->sx != 1 || p->oy != 0 || p->ox != 0 || p->gH != p->oH ||
             p->gW != p->oW || (p->oH & 1) || (p->oW & 1) || stride != 1 || p->y_coff != 0 || p->y_cstride != p->Cout)
             return P3D_UNSUPPORTED;
@@ -1013,67 +694,14 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     const int act = p->act == 1 ? 0 : (p->alpha >= 0.f && p->alpha <= 1.f ? 1 : 2);
     const bool clamp = p->clamp >= 0.f;
 
-    // 3 stages (96 KB at BN = 128): two CTAs per SM, so one tile's epilogue / TMA latency hides behind the other's MMAs.
-    // Grids that leave at most one CTA per SM anyway (the 4^2..32^2 backbone layers: 16-128 CTAs with 200+ k-steps each)
-    // are bound by TMA latency x bytes in flight instead; they get a 6-stage ring (192 KB).
     dim3 grid(tiles_m_total, ceil_div(p->Cout_padded, BN), p->B);
     const long base_ctas = (long)grid.x * grid.y * grid.z;
-    if (pair) {
-        a.splits = 1; a.partial = nullptr; a.Cout_pad = p->Cout_padded;
-        a.BN = 256;
-        a.idesc = tc::umma_idesc_f16(256, 256, 0);
-        const int n_tiles = tiles_m_total * tiles_n * p->B;
-        const size_t smem_q = kQStages * (size_t)(kBM * 128 + 128 * 128) + 256 + 2 * 512 * sizeof(float) + 1024;
-        int pairs = sm_count() / 2;
-        if (pairs > n_tiles) pairs = n_tiles;
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(2 * pairs, 1, 1);
-        cfg.blockDim = dim3(320, 1, 1);
-        cfg.dynamicSmemBytes = smem_q;
-        cfg.stream = (cudaStream_t)stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-#define P3D_LAUNCH_PAIR(ACT, CL)                                                                                              \
-    do {                                                                                                                      \
-        P3D_CUDA_TRY(cudaFuncSetAttribute(conv_gemm_pair_kernel<ACT, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
-                                          (int)smem_q));                                                                      \
-        P3D_CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_gemm_pair_kernel<ACT, CL>, tmA, tmB, a, n_tiles, tiles_n));                \
-    } while (0)
-        if (act == 0) { if (clamp) P3D_LAUNCH_PAIR(0, true); else P3D_LAUNCH_PAIR(0, false); }
-        else if (act == 1) { if (clamp) P3D_LAUNCH_PAIR(1, true); else P3D_LAUNCH_PAIR(1, false); }
-        else { if (clamp) P3D_LAUNCH_PAIR(2, true); else P3D_LAUNCH_PAIR(2, false); }
-#undef P3D_LAUNCH_PAIR
-        P3D_LAUNCH_CHECK();
-        return P3D_OK;
-    }
-    if (persist) {
-        a.splits = 1; a.partial = nullptr; a.Cout_pad = p->Cout_padded;
-        const int n_tiles = (int)base_ctas;
-        const size_t stage_bytes_p = 2 * (size_t)kBM * 128 + (size_t)BN * 128;
-        const size_t smem_p = kPStages * stage_bytes_p + 128 + 2 * 256 * sizeof(float) + 2 * 1024 * sizeof(float) + 1024;
-        const int ctas = n_tiles < sm_count() ? n_tiles : sm_count();
-#define P3D_LAUNCH_PERSIST(ACT, CL)                                                                                           \
-    do {                                                                                                                      \
-        P3D_CUDA_TRY(cudaFuncSetAttribute(conv_gemm_persist_kernel<ACT, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                          (int)smem_p));                                                                      \
-        conv_gemm_persist_kernel<ACT, CL><<<ctas, 320, smem_p, (cudaStream_t)stream>>>(tmA, tmB, a, n_tiles, tiles_n);        \
-    } while (0)
-        if (act == 0) { if (clamp) P3D_LAUNCH_PERSIST(0, true); else P3D_LAUNCH_PERSIST(0, false); }
-        else if (act == 1) { if (clamp) P3D_LAUNCH_PERSIST(1, true); else P3D_LAUNCH_PERSIST(1, false); }
-        else { if (clamp) P3D_LAUNCH_PERSIST(2, true); else P3D_LAUNCH_PERSIST(2, false); }
-#undef P3D_LAUNCH_PERSIST
-        P3D_LAUNCH_CHECK();
-        return P3D_OK;
-    }
-    // split-K for grids far smaller than the machine (4^2..16^2 layers: 16-32 CTAs each streaming 100-200 k-steps at
-    // the per-SM L2 ingest rate): every k-range becomes its own CTA writing raw fp32 partials into the caller's scratch
-    // buffer; conv_splitk_finish_kernel adds them in a fixed order and applies the epilogue. Two CTAs fit an SM, so the
-    // split count aims at two waves' worth of CTAs; every phase of a merged launch is split the same number of ways.
+    // split-K for grids far smaller than the machine (4^2..16^2 layers: 16-32 CTAs each streaming 100-200 k-steps): every
+    // k-range becomes its own CTA writing raw fp32 partials into the caller's scratch buffer; conv_splitk_finish_kernel adds
+    // them in a fixed order and applies the epilogue. The split count aims at one wave of CTAs (two for merged phases); every
+    // phase of a merged launch is split the same number of ways.
     a.splits = 1; a.partial = nullptr; a.Cout_pad = p->Cout_padded;
-    if (p->splitk_scratch && !p->up_prev && !p->residual && base_ctas * 2 <= sm_count() && min_total_k >= 8) {
+    if (p->splitk_scratch && !p->up_prev && !p->residual && !p->rgb_w && base_ctas * 2 <= sm_count() && min_total_k >= 8) {
         int splits = (int)((n_phases > 1 ? 2 * sm_count() : sm_count()) / base_ctas);
         if (splits > min_total_k / 4) splits = min_total_k / 4;
         if (splits > 16) splits = 16;
@@ -1091,21 +719,28 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
             }
         }
     }
+    // 4 stages by default; grids with at most one CTA per SM and long k-loops (the 4^2..32^2 backbone layers) are bound by
+    // TMA latency x bytes in flight instead and get the deepest ring the shared memory holds
     const bool deep = (long)grid.x * grid.y * grid.z <= sm_count() && max_total_k / a.splits > 6;
     const size_t stage_bytes = (size_t)kBM * 128 + (size_t)BN * 128;
-    const size_t smem = (deep ? 6 : 3) * stage_bytes + 64 + 2 * 128 * sizeof(float) + 1024 + (deep ? 64 : 0);
-#define P3D_LAUNCH_CONV_S(ST, ACT, CL)                                                                                        \
+    const int n_stages = deep ? kMaxStages : 4;
+    const size_t smem = n_stages * stage_bytes + 2 * kMaxStages * 8 + (2 * 128 + 8 * 128) * sizeof(float) + 1024;
+#define P3D_LAUNCH_CONV_N(ACT, CL, BNV)                                                                                       \
     do {                                                                                                                      \
-        P3D_CUDA_TRY(cudaFuncSetAttribute(conv_gemm_kernel<ST, ACT, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
+        P3D_CUDA_TRY(cudaFuncSetAttribute(conv_gemm_kernel<ACT, CL, BNV>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
                                           (int)smem));                                                                        \
-        conv_gemm_kernel<ST, ACT, CL><<<grid, 192, smem, (cudaStream_t)stream>>>(tmA, tmB, a);                                \
+        conv_gemm_kernel<ACT, CL, BNV><<<grid, kConvThreads, smem, (cudaStream_t)stream>>>(tmA, tmB, a, n_stages);           \
     } while (0)
 #define P3D_LAUNCH_CONV(ACT, CL)                                                                                              \
-    do { if (deep) P3D_LAUNCH_CONV_S(6, ACT, CL); else P3D_LAUNCH_CONV_S(3, ACT, CL); } while (0)
+    do {                                                                                                                      \
+        if (BN == 128) P3D_LAUNCH_CONV_N(ACT, CL, 128);                                                                       \
+        else if (BN == 64) P3D_LAUNCH_CONV_N(ACT, CL, 64);                                                                    \
+        else P3D_LAUNCH_CONV_N(ACT, CL, 32);                                                                                  \
+    } while (0)
     if (act == 0) { if (clamp) P3D_LAUNCH_CONV(0, true); else P3D_LAUNCH_CONV(0, false); }
     else if (act == 1) { if (clamp) P3D_LAUNCH_CONV(1, true); else P3D_LAUNCH_CONV(1, false); }
     else { if (clamp) P3D_LAUNCH_CONV(2, true); else P3D_LAUNCH_CONV(2, false); }
-#undef P3D_LAUNCH_CONV_S
+#undef P3D_LAUNCH_CONV_N
 #undef P3D_LAUNCH_CONV
     P3D_LAUNCH_CHECK();
     if (a.splits > 1) {

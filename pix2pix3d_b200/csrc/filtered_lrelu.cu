@@ -318,7 +318,7 @@ extern "C" int p3d_filtered_lrelu_act(void* x, unsigned char* s, int dtype, cons
     const int64_t total = (int64_t)((xmax + 3) >> 2) * ymax * planes;
     const int threads = 256;
     int64_t blocks = (total + threads - 1) / threads;
-    if (blocks > 148 * 64) blocks = 148 * 64;
+    if (blocks > (int64_t)sm_count() * 64) blocks = (int64_t)sm_count() * 64;
     if (blocks < 1) blocks = 1;
     const int sox = s_ofs ? s_ofs[0] : 0, soy = s_ofs ? s_ofs[1] : 0;
 #define P3D_FLA(M, T, A) filtered_lrelu_act_kernel<M, T, A><<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(               \

@@ -1,13 +1,13 @@
-// Tensor-core point query (sm_100a): ImportanceRenderer.run_model at free 3-D points -- tri-plane lookup, mean over the
+// Tensor-core point query (sm_90a): ImportanceRenderer.run_model at free 3-D points -- tri-plane lookup, mean over the
 // planes and the OSG decoder MLP, without a ray marcher (reference training/volumetric_rendering/renderer.py:142-148,
 // entered through TriPlane*Generator.sample / sample_mixed, training/triplane_cond.py:1063-1074, e.g. the 512^3 sigma
 // grid of applications/extract_mesh.py:60-81).
-//   * one CTA per SM, 384 threads = 3 groups of 128; a group walks 128-point tiles on its own (own mbarrier, own named
-//     barrier, own TMEM columns), so one group's gather overlaps another group's MMAs and epilogue;
+//   * one CTA per SM, 384 threads = 3 groups of 128 (warpgroups); a group walks 128-point tiles on its own (own named
+//     barrier), so one group's gather overlaps another group's MMAs and epilogue;
 //   * gather and decoder are the renderer's (render_tc.cuh): fp16 hi|lo feature rows in the SWIZZLE_128B K-major layout
-//     are the A operand of layer 1, hidden activations return to TMEM as packed fp16 hi/lo and feed layer 2 from there;
+//     are the A operand of layer 1, hidden activations stay in registers as packed fp16 hi/lo and feed layer 2 from there;
 //   * sigma is the fp32 dot of the hidden row with the sigma weights (as in the renderer's density passes);
-//   * colours are staged through the (now free) feature rows and leave as full 128-byte lines.
+//   * colours are staged through the (then free) feature rows and leave as full 128-byte lines.
 #include "render_tc.cuh"
 
 namespace p3d {
@@ -27,12 +27,9 @@ struct TcQueryParams {
 };
 
 constexpr int kQThreads = 384;
-constexpr int kQColsPerGroup = 160;     // D1: [0,128)  D2: [128,160)
 constexpr int kQOffFeat = kTcTail;                       // weight tiles first (1024-aligned base)
 constexpr int kQOffTail = kQOffFeat + 3 * 16384;
-constexpr int kQOffBar = kQOffTail + kTcTailFloats * 4;  // 3 mbarriers + the TMEM base
-constexpr int kQSmemBytes = kQOffBar + 3 * 8 + 16;
-static_assert(kQOffBar % 8 == 0, "mbarrier alignment");
+constexpr int kQSmemBytes = kQOffTail + kTcTailFloats * 4;
 
 __global__ void __launch_bounds__(kQThreads, 1) run_model_tc_kernel(const TcQueryParams P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -44,8 +41,6 @@ __global__ void __launch_bounds__(kQThreads, 1) run_model_tc_kernel(const TcQuer
     uint8_t* tile = smem + kQOffFeat + grp * 16384;
     const float* tail = reinterpret_cast<const float*>(smem + kQOffTail);
     const float* b1 = tail, *b2c = tail + 128, *b2s = tail + 192, *w2s = tail + 196;
-    uint64_t* mma_bar = reinterpret_cast<uint64_t*>(smem + kQOffBar);
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(mma_bar + 3);
 
     {
         const uint4* src = reinterpret_cast<const uint4*>(P.decoder_packed);
@@ -55,28 +50,13 @@ __global__ void __launch_bounds__(kQThreads, 1) run_model_tc_kernel(const TcQuer
         float* tdst = reinterpret_cast<float*>(smem + kQOffTail);
         for (int i = tid; i < kTcTailFloats; i += kQThreads) tdst[i] = __ldg(tsrc + i);
     }
-    if (tid == 0) {
-        for (int g = 0; g < 3; ++g) tc::mbar_init(&mma_bar[g], 1);
-        tc::fence_barrier_init();
-    }
-    if (warp == 0) tc::tmem_alloc(tmem_ptr_smem, 512);
     tc::fence_proxy_async();          // weight tiles were written through the generic proxy
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_grp = *tmem_ptr_smem + (uint32_t)(grp * kQColsPerGroup);
-    const uint32_t tmem_row = tmem_grp + ((uint32_t)(q * 32) << 16);
-    uint32_t bar_phase = 0;
     const uint32_t w1a = tc::smem_u32(smem + kTcW1A), w1b = tc::smem_u32(smem + kTcW1B);
     const bool colours = P.out_rgb != nullptr;      // sigma-only query (mesh extraction): layer 1 of the sigma net + one dot
-    const uint32_t idesc_l1 = (colours && n_nets == 2) ? tc::umma_idesc_f16(128, 128, 0) : tc::umma_idesc_f16(128, 64, 0);
-    const int l1_row0 = colours ? 0 : sig * 64;     // first W1 row (= hidden unit) layer 1 computes
-    const uint32_t idesc_n32 = tc::umma_idesc_f16(128, 32, 0);
     const uint32_t tile32 = tc::smem_u32(tile);
     const TcPlaneView pv{P.planes, P.H, P.W, P.img_stride, P.plane_stride, P.pix_stride};
-
-    auto group_sync = [&]() { tc::tc_fence_before(); tc::named_bar_sync(1 + grp, 128); tc::tc_fence_after(); };
-    auto wait_mma = [&]() { tc::mbar_wait(&mma_bar[grp], bar_phase); bar_phase ^= 1; tc::tc_fence_after(); };
+    auto group_sync = [&]() { tc::named_bar_sync(1 + grp, 128); };
 
     for (long long t = (long long)blockIdx.x * 3 + grp; t < P.n_tiles; t += (long long)gridDim.x * 3) {
         const long long p = t * 128 + m;
@@ -92,81 +72,43 @@ __global__ void __launch_bounds__(kQThreads, 1) run_model_tc_kernel(const TcQuer
         }
         tc_gather_rows(pv, tile, q, lane, v, b, px, py, pz);
         tc::fence_proxy_async();
-        group_sync();                  // all 128 rows written; every warp is done with D1 / D2 of the previous tile
-        if (m == 0) {
-            // layer 1: D1[:, 0:64*n_nets) = [hi|lo] x [Whi|Whi]^T + [hi|lo] x [Wlo|0]^T
-            const uint64_t da = tc::umma_desc_k128(tile32);
-            const uint64_t dba = tc::umma_desc_k128(w1a + l1_row0 * 128), dbb = tc::umma_desc_k128(w1b + l1_row0 * 128);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc::umma_f16(tmem_grp, da + 2 * k, dba + 2 * k, idesc_l1, k != 0);
-#pragma unroll
-            for (int k = 0; k < 2; ++k) tc::umma_f16(tmem_grp, da + 2 * k, dbb + 2 * k, idesc_l1, 1);
-            tc::umma_commit(&mma_bar[grp]);
-        }
-        wait_mma();                    // the feature rows are free from here on (used as the colour staging rows below)
-        float sg0 = b2s[sig], sg1 = 0.f;
+        group_sync();                  // all 128 rows written
+        float sg[2][2];
+        float d2[2][2][16];
         if (!colours) {
-            // D1[:, 0:64) holds the sigma net's hidden pre-activations: sigma = w2[0] . softplus(h) + b2[0]
+            DecHidden hd;
+            dec_hidden<true>(tile32, w1a, w1b, sig, b1, w2s, b2s, lane, hd, sg);
+        } else {
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                uint32_t vv[32];
-                tc::tmem_ld_32x32(tmem_row + half * 32, vv);
-                tc::tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                    const int jj = sig * 64 + half * 32 + j;
-                    sg0 = fmaf(w2s[jj], softplus2(__uint_as_float(vv[j]) + b1[jj]), sg0);
-                    sg1 = fmaf(w2s[jj + 1], softplus2(__uint_as_float(vv[j + 1]) + b1[jj + 1]), sg1);
-                }
+            for (int net = 0; net < 2; ++net) {
+                if (net >= n_nets) break;
+                DecHidden hd;
+                float sn[2][2];
+                if (net == sig) dec_hidden<true>(tile32, w1a, w1b, net, b1, w2s, b2s, lane, hd, sg);
+                else dec_hidden<false>(tile32, w1a, w1b, net, b1, w2s, b2s, lane, hd, sn);
+                dec_colours(hd, tc::smem_u32(smem + kTcW2H + net * 8192), tc::smem_u32(smem + kTcW2L + net * 8192), d2[net]);
             }
         }
-#pragma unroll 1
-        for (int net = 0; colours && net < n_nets; ++net) {
-            // hidden: D1[:, net*64 .. +64) -> softplus -> packed fp16 hi (32 cols) | lo (32 cols), in place
-            uint32_t ph[32], pl[32];
-            const bool is_sig = net == sig;
+        if ((lane & 3) == 0) {
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                uint32_t vv[32];
-                tc::tmem_ld_32x32(tmem_row + net * 64 + half * 32, vv);
-                tc::tmem_ld_wait();
+            for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                    const int jj = net * 64 + half * 32 + j;
-                    const float h0 = softplus2(__uint_as_float(vv[j]) + b1[jj]);
-                    const float h1 = softplus2(__uint_as_float(vv[j + 1]) + b1[jj + 1]);
-                    if (is_sig) { sg0 = fmaf(w2s[jj], h0, sg0); sg1 = fmaf(w2s[jj + 1], h1, sg1); }
-                    const __half2 hh = __floats2half2_rn(h0, h1);
-                    const float2 back = __half22float2(hh);
-                    const __half2 ll = __floats2half2_rn(h0 - back.x, h1 - back.y);
-                    ph[half * 16 + j / 2] = *reinterpret_cast<const uint32_t*>(&hh);
-                    pl[half * 16 + j / 2] = *reinterpret_cast<const uint32_t*>(&ll);
+                for (int h = 0; h < 2; ++h) {
+                    const long long pr = t * 128 + dec_frag_row(mb, h, q, lane);
+                    if (pr < P.total) P.out_sigma[pr] = sg[mb][h];
                 }
-            }
-            tc::tmem_st_32x32(tmem_row + net * 64, ph);
-            tc::tmem_st_32x32(tmem_row + net * 64 + 32, pl);
-            tc::tmem_st_wait();
+        }
+        group_sync();                  // every warp's MMAs have read the feature rows: they are the colour staging rows now
+#pragma unroll
+        for (int net = 0; net < 2; ++net) {
+            if (!colours || net >= n_nets) break;
+            dec_stage_rows(d2[net], tile, q, lane);
             group_sync();
-            if (m == 0) {
-                // layer 2: D2 = A2hi*W2hi + A2lo*W2hi + A2hi*W2lo, A2 packed fp16 in TMEM cols [net*64, net*64+64)
-                const uint32_t ahi = tmem_grp + net * 64, alo = ahi + 32, d2 = tmem_grp + 128;
-                const uint64_t bh = tc::umma_desc_k128(tc::smem_u32(smem + kTcW2H + net * 8192));
-                const uint64_t bl = tc::umma_desc_k128(tc::smem_u32(smem + kTcW2L + net * 8192));
-#pragma unroll
-                for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, ahi + 8 * k, bh + 2 * k, idesc_n32, k != 0);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, alo + 8 * k, bh + 2 * k, idesc_n32, 1);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, ahi + 8 * k, bl + 2 * k, idesc_n32, 1);
-                tc::umma_commit(&mma_bar[grp]);
-            }
-            wait_mma();
             uint32_t cv[32];
-            tc::tmem_ld_32x32(tmem_row + 128, cv);
-            tc::tmem_ld_wait();
+            dec_read_row(tile, m, cv);
             const uint32_t smask = net == 0 ? P.mask[0] : P.mask[1];
-            // stage this row's 32 colours in its feature row (16-byte chunks XOR-swizzled by the row), then let the warp
-            // write its 32 rows as 128-byte lines: 4 rows per instruction, lane = 4 consecutive channels
+            // this row's 32 colours go back to its staging row, then the warp writes its 32 rows as 128-byte lines: 4 rows per
+            // instruction, lane = 4 consecutive channels
             const uint32_t rb = tile32 + (uint32_t)m * 128, swx = (uint32_t)(m & 7) << 4;
 #pragma unroll
             for (int i = 0; i < 32; i += 4) {
@@ -188,16 +130,8 @@ __global__ void __launch_bounds__(kQThreads, 1) run_model_tc_kernel(const TcQuer
                 const uint4 val = lds_u4((tile32 + (uint32_t)row * 128) | (((uint32_t)cq << 4) ^ ((uint32_t)(row & 7) << 4)));
                 if (pr < P.total) *reinterpret_cast<uint4*>(P.out_rgb + pr * cout + net * kOut + cq * 4) = val;
             }
-            __syncwarp();              // rows are rewritten by the next net / the next tile's taps
+            group_sync();              // rows are rewritten by the next net / the next tile's taps
         }
-        if (v) P.out_sigma[p] = sg0 + sg1;
-    }
-
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(*tmem_ptr_smem, 512);
     }
 }
 

@@ -1,4 +1,4 @@
-// Fused volumetric renderer for sm_100a: tri-plane gather + OSG decoder MLP + ray marching +
+// Fused volumetric renderer for sm_90a: tri-plane gather + OSG decoder MLP + ray marching +
 // importance resampling + merge, replacing the ~60 ATen launches of
 // training/volumetric_rendering/renderer.py:88-253 and ray_marcher.py:25-57 (reference repo).
 //
@@ -725,8 +725,8 @@ __global__ void __launch_bounds__(128) sample_importance_kernel(const float* __r
 // may drive several devices)
 int sm_count() {
     int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
     return n;
 }
 
@@ -737,7 +737,7 @@ using namespace p3d;
 extern "C" {
 
 int p3d_abi_version(void) { return 5; }
-const char* p3d_build_info(void) { return "libp3d sm_100a " __DATE__ " " __TIME__; }
+const char* p3d_build_info(void) { return "libp3d sm_90a " __DATE__ " " __TIME__; }
 const char* p3d_status_string(int status) {
     if (status == P3D_OK) return "ok";
     if (status == P3D_UNSUPPORTED) return "unsupported configuration";

@@ -1,4 +1,4 @@
-// Device functions shared by the two fused renderers (render.cu: fp32 CUDA-core decoder; render_tc.cu: tcgen05 decoder):
+// Device functions shared by the two fused renderers (render.cu: fp32 CUDA-core decoder; render_tc.cu: wgmma decoder):
 // tri-plane bilinear taps, MipRayMarcher2 weights per ray, importance-sampling bookkeeping.
 #pragma once
 #include "p3d_common.cuh"

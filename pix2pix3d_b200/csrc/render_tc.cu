@@ -1,18 +1,16 @@
-// Fused volumetric renderer, tensor-core decoder variant (sm_100a): same pipeline and bookkeeping as render.cu
+// Fused volumetric renderer, tensor-core decoder variant (sm_90a): same pipeline and bookkeeping as render.cu
 // (reference training/volumetric_rendering/renderer.py:88-253, ray_marcher.py:25-57), with the OSG decoder MLP on
-// tcgen05:
-//   * one CTA per SM, 384 threads = 3 groups of 128; a group owns 128 sample rows (= the 128 TMEM lanes of an M=128
-//     MMA) of the CTA's ray tile for the coarse pass and 128 rows for the fine pass;
+// wgmma:
+//   * one CTA per SM, 384 threads = 3 groups of 128 (warpgroups); a group owns 128 sample rows of the CTA's ray tile for the
+//     coarse pass and 128 rows for the fine pass (two M=64 MMAs each);
 //   * gathered features are written as fp16 (hi | lo) into 128-byte shared-memory rows in the SWIZZLE_128B K-major
 //     layout, so the feature store IS the A operand of layer 1:  [hi|lo] x [Whi|Whi]^T + [hi|lo] x [Wlo|0]^T
-//     = hi*Whi + lo*Whi + hi*Wlo (fp32 accumulate in TMEM, error ~2^-22);
-//   * hidden activations go TMEM -> registers (softplus) -> TMEM as packed fp16 hi/lo and feed layer 2 straight
-//     from TMEM (A-from-TMEM MMA), three passes again; colours come back with tcgen05.ld and are reduced per ray
-//     with warp shuffles using the coefficient form rgb = sum_j c_j (w_{j-1} + w_j)/2.
-//   The density pre-passes (coarse / fine) run layer 1 of the sigma net on the tensor core, take sigma as a 64-term fp32
-//   dot of the hidden row and -- since that net's softplus'd hidden row is in registers anyway -- pack it and issue ITS
-//   layer 2 right there: the 32 colour pre-activations of the sigma net stay parked in TMEM (32 columns per tile) until the
-//   ray's weights are known, so the colour pass evaluates only the OTHER net (64 instead of 128 softplus per sample).
+//     = hi*Whi + lo*Whi + hi*Wlo (fp32 accumulate in registers, error ~2^-22);
+//   * hidden activations go accumulator registers -> softplus -> packed fp16 hi/lo registers, which are the A operand of
+//     layer 2 (three passes again); colours are parked in the feature rows of the pass (free by then), read back one row per
+//     thread and reduced per ray with warp shuffles using the coefficient form rgb = sum_j c_j (w_{j-1} + w_j)/2.
+//   The density pre-passes (coarse / fine) run layer 1 of the sigma net and take sigma as a 64-term fp32 dot of each hidden
+//   row; the colour pass evaluates both nets on the tile of the pass.
 #include <cstdlib>
 #include <type_traits>
 #include "render_tc.cuh"
@@ -59,7 +57,7 @@ __global__ void pack_decoder_tc_kernel(PackTcArgs a, uint8_t* __restrict__ out) 
 // ---- shared-memory plan ----------------------------------------------------------------------------------
 struct TcLayout {
     int RT, Sc, Sf, S, gc, gf, NGc, NGf, tiles_c, tiles_f;
-    int off_feat, off_tail, off_ray, ray_stride, off_part, off_scal, off_bar, total_bytes;
+    int off_feat, off_tail, off_ray, ray_stride, off_part, off_scal, total_bytes;
     int o_dC, o_sC, o_dF, o_sF, o_sd, o_ss, o_w, o_cdf, o_om;
 };
 
@@ -86,8 +84,6 @@ __host__ __device__ inline TcLayout make_tc_layout(int RT, int Sc, int Sf, int n
     L.off_ray = o; o += RT * r * 4;
     L.off_part = o; o += RT * (L.NGc + L.NGf) * (kOut * n_nets) * 4;
     L.off_scal = o; o += (4 * RT + 4) * 4;
-    o = round_up(o, 8);
-    L.off_bar = o; o += 3 * 8 + 16;
     L.total_bytes = o;
     return L;
 }
@@ -101,10 +97,6 @@ struct TcRenderParams {
 
 
 constexpr int kTcThreads = 384;
-// TMEM columns of a group: D1 [0,64) hidden pre-activations / packed hidden of the net in flight; [64,96) parked colour
-// pre-activations of the sigma net, coarse tile; [96,128) the same for the fine tile; D2 [128,160) colours of the other net
-constexpr int kTcColsPerGroup = 160;
-constexpr int kTcColPark = 64, kTcColD2 = 128;
 
 __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRenderParams P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -113,7 +105,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
     const p3d_render_args_t& a = P.a;
     const TcLayout& L = P.L;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = kTcThreads >> 5;
-    const int grp = tid >> 7, m = tid & 127, q = warp & 3;       // group, row inside the group's tile, TMEM lane quarter
+    // group (warpgroup), row inside the group's tile, warp of the group. The group index is broadcast from lane 0 so that the
+    // compiler sees it warp-uniform: the per-group branches around the decoder's wgmma are then not divergent paths, which
+    // would make ptxas serialise every wgmma of the kernel
+    const int grp = __shfl_sync(0xffffffffu, tid >> 7, 0), m = tid & 127, q = warp & 3;
     const int RT = L.RT, Sc = L.Sc, Sf = L.Sf, S = L.S, n_nets = a.n_nets;
 
     uint8_t* feat = smem + L.off_feat;
@@ -123,10 +118,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
     float* part = reinterpret_cast<float*>(smem + L.off_part);
     float* scal = reinterpret_cast<float*>(smem + L.off_scal);
     uint32_t* cta_keys = reinterpret_cast<uint32_t*>(scal + 4 * RT);
-    uint64_t* mma_bar = reinterpret_cast<uint64_t*>(smem + L.off_bar);
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(mma_bar + 3);
 
-    // ---- one-time setup: weights -> smem, barriers, TMEM ------------------------------------------------
+    // ---- one-time setup: weights -> smem ------------------------------------------------
     {
         const uint4* src = reinterpret_cast<const uint4*>(a.decoder_packed);
         uint4* dst = reinterpret_cast<uint4*>(smem);
@@ -135,86 +128,34 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
         float* tdst = reinterpret_cast<float*>(smem + L.off_tail);
         for (int i = tid; i < kTcTailFloats; i += kTcThreads) tdst[i] = __ldg(tsrc + i);
     }
-    if (tid == 0) {
-        for (int g = 0; g < 3; ++g) tc::mbar_init(&mma_bar[g], 1);
-        tc::fence_barrier_init();
-        cta_keys[0] = 0u; cta_keys[1] = 0u;
-    }
-    if (warp == 0) tc::tmem_alloc(tmem_ptr_smem, 512);
+    if (tid == 0) { cta_keys[0] = 0u; cta_keys[1] = 0u; }
     tc::fence_proxy_async();          // weight tiles were written through the generic proxy
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_grp = *tmem_ptr_smem + (uint32_t)(grp * kTcColsPerGroup);
-    const uint32_t tmem_row = tmem_grp + ((uint32_t)(q * 32) << 16);      // this thread's lane quarter
-    uint32_t bar_phase = 0;
     const uint32_t w1a = tc::smem_u32(smem + kTcW1A), w1b = tc::smem_u32(smem + kTcW1B);
-    const uint32_t idesc_n64 = tc::umma_idesc_f16(128, 64, 0), idesc_n32 = tc::umma_idesc_f16(128, 32, 0);
     const int sig = a.sigma_net;
-
-    // layer 1 on this group's feature tile: D1[:, 0:ncols) = [hi|lo] x W^T   (issued by the group leader)
-    auto issue_layer1 = [&](int tile, int row0, uint32_t idesc) {
-        const uint32_t fa = tc::smem_u32(feat + tile * 16384);
-        const uint64_t da = tc::umma_desc_k128(fa);
-        const uint64_t dba = tc::umma_desc_k128(w1a + row0 * 128), dbb = tc::umma_desc_k128(w1b + row0 * 128);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16(tmem_grp, da + 2 * k, dba + 2 * k, idesc, k != 0);   // hi*Whi + lo*Whi
-#pragma unroll
-        for (int k = 0; k < 2; ++k) tc::umma_f16(tmem_grp, da + 2 * k, dbb + 2 * k, idesc, 1);        // hi*Wlo
-        tc::umma_commit(&mma_bar[grp]);
-    };
-    // layer 2 for one net: D[dcol, dcol+32) = A2hi*W2hi + A2lo*W2hi + A2hi*W2lo, A2 packed fp16 in TMEM cols [0, 64)
-    auto issue_layer2 = [&](int net, int dcol) {
-        const uint32_t ahi = tmem_grp, alo = ahi + 32, d2 = tmem_grp + dcol;
-        const uint64_t bh = tc::umma_desc_k128(tc::smem_u32(smem + kTcW2H + net * 8192));
-        const uint64_t bl = tc::umma_desc_k128(tc::smem_u32(smem + kTcW2L + net * 8192));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, ahi + 8 * k, bh + 2 * k, idesc_n32, k != 0);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, alo + 8 * k, bh + 2 * k, idesc_n32, 1);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, ahi + 8 * k, bl + 2 * k, idesc_n32, 1);
-        tc::umma_commit(&mma_bar[grp]);
-    };
-    auto group_sync = [&]() { tc::tc_fence_before(); tc::named_bar_sync(1 + grp, 128); tc::tc_fence_after(); };
-    auto wait_mma = [&]() { tc::mbar_wait(&mma_bar[grp], bar_phase); bar_phase ^= 1; tc::tc_fence_after(); };
+    auto group_sync = [&]() { tc::named_bar_sync(1 + grp, 128); };
 
     // warp-cooperative gather of this warp's 32 rows into feature tile `tile` (render_tc.cuh)
     auto gather_rows = [&](int tile, bool valid, int b, float px, float py, float pz) {
         const TcPlaneView pv{a.planes_nhwc, a.H, a.W, P.img_stride, P.plane_stride, P.pix_stride};
         tc_gather_rows(pv, feat + tile * 16384, q, lane, valid, b, px, py, pz);
     };
-    // hidden row of `net` (pre-activations in D1[:, 0:64)) -> softplus -> packed fp16 hi (cols 0..31) | lo (cols 32..63) in
-    // place = the A operand of layer 2; with WANT_SIGMA also sigma = the fp32 dot with the sigma row of W2 (returned)
-    auto hidden_to_tmem = [&](int net, auto want_sigma) -> float {
-        constexpr bool kSigma = decltype(want_sigma)::value;
-        uint32_t ph[32], pl[32];
-        float acc0 = kSigma ? b2s[net] : 0.f, acc1 = 0.f;
+    // density of every row of feature tile `tile` this thread owns a fragment of -> the ray buffer. Row r of the group is
+    // sample (grp * 128 + r) of the tile's rays, n samples per ray, stored at offset o_s of the ray.
+    auto density = [&](int tile, int n, int o_s, int ray0) {
+        DecHidden hd;
+        float sg[2][2];
+        dec_hidden<true>(tc::smem_u32(feat + tile * 16384), w1a, w1b, sig, b1, w2s, b2s, lane, hd, sg);
+        if ((lane & 3) == 0) {
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            uint32_t vv[32];
-            tc::tmem_ld_32x32(tmem_row + half * 32, vv);
-            tc::tmem_ld_wait();
+            for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-            for (int j = 0; j < 32; j += 2) {
-                const int jj = net * 64 + half * 32 + j;
-                const float h0 = softplus2(__uint_as_float(vv[j]) + b1[jj]);
-                const float h1 = softplus2(__uint_as_float(vv[j + 1]) + b1[jj + 1]);
-                if (kSigma) { acc0 = fmaf(w2s[jj], h0, acc0); acc1 = fmaf(w2s[jj + 1], h1, acc1); }
-                const __half2 hh = __floats2half2_rn(h0, h1);
-                const float2 back = __half22float2(hh);
-                const __half2 ll = __floats2half2_rn(h0 - back.x, h1 - back.y);
-                ph[half * 16 + j / 2] = *reinterpret_cast<const uint32_t*>(&hh);
-                pl[half * 16 + j / 2] = *reinterpret_cast<const uint32_t*>(&ll);
-            }
+                for (int h = 0; h < 2; ++h) {
+                    const int i = grp * 128 + dec_frag_row(mb, h, q, lane), r = i / n;
+                    if (r < RT && ray0 + r < P.total_rays) rayb[r * L.ray_stride + o_s + i % n] = sg[mb][h];
+                }
         }
-        tc::tmem_st_32x32(tmem_row, ph);
-        tc::tmem_st_32x32(tmem_row + 32, pl);
-        tc::tmem_st_wait();
-        return acc0 + acc1;
     };
-    const std::true_type with_sigma{};
-    const std::false_type no_sigma{};
 
     for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
         const int ray0 = tile * RT;
@@ -233,7 +174,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
 
         // ---- P1/P2: coarse gather + sigma -------------------------------------------------------------
         float dC = 0.f;
-        bool park_pending = false;
         if (grpC) {
             float px = 0.f, py = 0.f, pz = 0.f;
             if (vC) {
@@ -247,17 +187,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
             gather_rows(grp, vC, bC, px, py, pz);
             tc::fence_proxy_async();
             group_sync();
-            if (m == 0) issue_layer1(grp, sig * 64, idesc_n64);
-            wait_mma();
-            const float sg = hidden_to_tmem(sig, with_sigma);
-            if (vC) { rbC[L.o_dC + sC] = dC; rbC[L.o_sC + sC] = sg; }
-            group_sync();                                           // every row of the tile has its packed hidden in TMEM
-            if (m == 0) issue_layer2(sig, kTcColPark);              // colours of the sigma net, parked until the colour pass
-            park_pending = true;                                    // its commit is consumed before the next commit is issued
+            density(grp, Sc, L.o_sC, ray0);
+            if (vC) rbC[L.o_dC + sC] = dC;
         }
-        tc::tc_fence_before();
         __syncthreads();
-        tc::tc_fence_after();
 
         // ---- P3: coarse march + importance cdf (warp per ray) ---------------------------------------------
         float dF = 0.f;
@@ -299,19 +232,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
                 }
                 gather_rows(L.tiles_c + grp, vF, bF, px, py, pz);
                 tc::fence_proxy_async();
-                if (park_pending) { wait_mma(); park_pending = false; }     // the coarse tile's parked layer 2 (long done)
                 group_sync();
-                if (m == 0) issue_layer1(L.tiles_c + grp, sig * 64, idesc_n64);
-                wait_mma();
-                const float sg = hidden_to_tmem(sig, with_sigma);
-                if (vF) { rbF[L.o_dF + sF] = dF; rbF[L.o_sF + sF] = sg; }
-                group_sync();
-                if (m == 0) issue_layer2(sig, kTcColPark + 32);
-                park_pending = true;
+                density(L.tiles_c + grp, Sf, L.o_sF, ray0);
+                if (vF) rbF[L.o_dF + sF] = dF;
             }
-            tc::tc_fence_before();
             __syncthreads();
-            tc::tc_fence_after();
         }
 
         // ---- P5: stable rank merge (renderer.py:157-167) -------------------------------------------------
@@ -399,12 +324,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
                 const float wl = rank > 0 ? rb[L.o_w + rank - 1] : 0.f;
                 coef = 0.5f * (wl + rb[L.o_w + rank]);
             }
-            // colour pre-activations of one net (32 TMEM columns at `col`) -> bias, sigmoid where masked, x coefficient,
+            // colour pre-activations of one net (this thread's row) -> bias, sigmoid where masked, x coefficient,
             // reduction over the rows of a ray segment -> per-segment partial sums in shared memory
-            auto colour_epilogue = [&](int net, int col) {
-                uint32_t cv[32];
-                tc::tmem_ld_32x32(tmem_row + col, cv);
-                tc::tmem_ld_wait();
+            auto colour_epilogue = [&](int net, const uint32_t (&cv)[32]) {
                 const uint32_t smask = a.sigmoid_mask[net];
                 float acc[32];
                 // the mask is all-or-nothing per net for every shipped decoder (rgb: sigmoid; semantic: raw logits when there are
@@ -458,24 +380,30 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
                     }
                 }
             };
-            if (park_pending) { wait_mma(); park_pending = false; }      // the last parked layer 2 has landed
-            const int oth = 1 - sig;
-            // the other net's layer 1 runs under the epilogue of the parked colours. D1 is free: every row's packed hidden was
-            // consumed by a layer 2 this thread has waited for, and MMAs of one issuer execute in order
-            if (n_nets == 2 && m == 0) issue_layer1((pass == 0 ? 0 : L.tiles_c) + grp, oth * 64, idesc_n64);
-            colour_epilogue(sig, kTcColPark + pass * 32);
-            if (n_nets == 2) {
-                wait_mma();
-                hidden_to_tmem(oth, no_sigma);
+            // colour pre-activations of both nets from this pass's feature tile, then the tile is their staging area
+            uint8_t* ftile = feat + ((pass == 0 ? 0 : L.tiles_c) + grp) * 16384;
+            float d2[2][2][16];
+#pragma unroll
+            for (int net = 0; net < 2; ++net) {
+                if (net >= n_nets) break;
+                DecHidden hd;
+                float sn[2][2];
+                dec_hidden<false>(tc::smem_u32(ftile), w1a, w1b, net, b1, w2s, b2s, lane, hd, sn);
+                dec_colours(hd, tc::smem_u32(smem + kTcW2H + net * 8192), tc::smem_u32(smem + kTcW2L + net * 8192), d2[net]);
+            }
+            group_sync();          // every warp's MMAs have read the feature tile
+#pragma unroll
+            for (int net = 0; net < 2; ++net) {
+                if (net >= n_nets) break;
+                dec_stage_rows(d2[net], ftile, q, lane);
                 group_sync();
-                if (m == 0) issue_layer2(oth, kTcColD2);
-                wait_mma();
-                colour_epilogue(oth, kTcColD2);
+                uint32_t cv[32];
+                dec_read_row(ftile, m, cv);
+                colour_epilogue(net, cv);
+                group_sync();      // the staging rows are rewritten by the next net
             }
         }
-        tc::tc_fence_before();
         __syncthreads();
-        tc::tc_fence_after();
         {
             const int NG = L.NGc + L.NGf;
             for (int i = tid; i < RT * P.cout; i += kTcThreads) {
@@ -494,12 +422,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
     // ---- global depth clamp (ray_marcher.py:49-50) -----------------------------------------------------------
     __shared__ bool is_last;
     __threadfence();
-    tc::tc_fence_before();
     __syncthreads();
-    if (warp == 0) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(*tmem_ptr_smem, 512);
-    }
     if (tid == 0) {
         atomicMax(a.workspace + 0, cta_keys[0]);
         atomicMax(a.workspace + 1, cta_keys[1]);

@@ -1,8 +1,9 @@
-// Pieces shared by the tensor-core renderer (render_tc.cu) and the tensor-core point query (query_tc.cu): the packed
-// decoder image, the SWIZZLE_128B row addressing and the shared-memory / global load-store helpers.
+// Pieces shared by the tensor-core renderers (render_tc.cu, render_tc2.cu) and the tensor-core point query (query_tc.cu):
+// the packed decoder image, the SWIZZLE_128B row addressing, the shared-memory / global load-store helpers and the decoder
+// MLP of one 128-row tile on wgmma.
 #pragma once
 #include "render_common.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 
 namespace p3d {
 
@@ -134,6 +135,118 @@ __device__ __forceinline__ void tc_gather_rows(const TcPlaneView& pv, uint8_t* t
         if (ok) fetch4(q * 32 + r, f);                           // 12 x 16 B per lane in flight
         __syncwarp();            // every lane has read the parked taps before the rows are overwritten
         if (ok) store4(q * 32 + r, f);
+    }
+}
+
+// ---- decoder MLP of one 128-row tile on wgmma (a group of 128 threads = one warpgroup) ---------------------------------
+// Fragment ownership: thread (warp wq of the group, lane l) holds tile rows 64 mb + 16 wq + 8 h + l/4 (mb, h in {0, 1}).
+__device__ __forceinline__ int dec_frag_row(int mb, int h, int wq, int lane) { return 64 * mb + 16 * wq + 8 * h + (lane >> 2); }
+
+// softplus'd hidden row of one net as the fp16 hi / lo A operand of layer 2: [mb][k-step][register]
+struct DecHidden {
+    uint32_t hi[2][4][4], lo[2][4][4];
+};
+
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+    const __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// Layer 1 of `net` on the feature tile at shared address `fa`:  [hi|lo] x [Whi|Whi]^T + [hi|lo] x [Wlo|0]^T (fp32 accumulate),
+// softplus, and the split into fp16 hi + lo. With kSigma also sigma = b2[0] + the fp32 dot of each owned hidden row with
+// the sigma row of W2: sig[mb][h], complete in every lane of the quad that owns the row.
+template <bool kSigma>
+__device__ __forceinline__ void dec_hidden(uint32_t fa, uint32_t w1a, uint32_t w1b, int net, const float* b1, const float* w2s,
+                                           const float* b2s, int lane, DecHidden& hd, float (&sig)[2][2]) {
+    const uint64_t dba = tc::wgmma_desc_k128(w1a + (uint32_t)net * 64 * 128), dbb = tc::wgmma_desc_k128(w1b + (uint32_t)net * 64 * 128);
+    const int c = 2 * (lane & 3);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+        float acc[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+        const uint64_t da = tc::wgmma_desc_k128(fa + (uint32_t)mb * 64 * 128);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_ss(acc, da + 2 * k, dba + 2 * k);      // hi*Whi + lo*Whi
+#pragma unroll
+        for (int k = 0; k < 2; ++k) tc::wgmma_ss(acc, da + 2 * k, dbb + 2 * k);      // hi*Wlo
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::wgmma_hold(acc);
+        float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int jj = net * 64 + 8 * i + c + e;
+                const float h0 = softplus2(acc[4 * i + e] + b1[jj]), h1 = softplus2(acc[4 * i + 2 + e] + b1[jj]);
+                if (kSigma) { s0 = fmaf(w2s[jj], h0, s0); s1 = fmaf(w2s[jj], h1, s1); }
+                acc[4 * i + e] = h0; acc[4 * i + 2 + e] = h1;
+            }
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const float x0 = acc[8 * kk + 2 * r], x1 = acc[8 * kk + 2 * r + 1];
+                const uint32_t h = pack_half2(x0, x1);
+                const float2 back = __half22float2(*reinterpret_cast<const __half2*>(&h));
+                hd.hi[mb][kk][r] = h;
+                hd.lo[mb][kk][r] = pack_half2(x0 - back.x, x1 - back.y);
+            }
+        if (kSigma) {
+            s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+            s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+            sig[mb][0] = b2s[net] + s0; sig[mb][1] = b2s[net] + s1;
+        }
+    }
+}
+
+// Layer 2 of `net`: colour pre-activations D2[128 x 32] = A2hi*W2hi + A2lo*W2hi + A2hi*W2lo (A2 from registers)
+__device__ __forceinline__ void dec_colours(const DecHidden& hd, uint32_t w2h, uint32_t w2l, float (&d)[2][16]) {
+    const uint64_t bh = tc::wgmma_desc_k128(w2h), bl = tc::wgmma_desc_k128(w2l);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) d[mb][i] = 0.f;
+    tc::wgmma_fence();
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_rs(d[mb], hd.hi[mb][k], bh + 2 * k);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_rs(d[mb], hd.lo[mb][k], bh + 2 * k);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_rs(d[mb], hd.hi[mb][k], bl + 2 * k);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::wgmma_hold(d[0]);
+    tc::wgmma_hold(d[1]);
+}
+
+// The colour fragments -> fp32 rows of 32 in a 16 KB tile (16-byte chunks XOR-swizzled by the row), so that thread m of the
+// group can read row m with dec_read_row. The caller synchronises the group between the two.
+__device__ __forceinline__ void dec_stage_rows(const float (&d)[2][16], uint8_t* tile, int wq, int lane) {
+    const int c = 2 * (lane & 3);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = dec_frag_row(mb, h, wq, lane);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int col = 8 * i + c;
+                *reinterpret_cast<float2*>(tile + row * 128 + ((((col >> 2) ^ (row & 7)) << 4) | ((col & 3) << 2))) =
+                    make_float2(d[mb][4 * i + 2 * h], d[mb][4 * i + 2 * h + 1]);
+            }
+        }
+}
+__device__ __forceinline__ void dec_read_row(const uint8_t* tile, int m, uint32_t (&v)[32]) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const uint4 t = *reinterpret_cast<const uint4*>(tile + m * 128 + ((j ^ (m & 7)) << 4));
+        v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
     }
 }
 

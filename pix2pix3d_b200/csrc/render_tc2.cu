@@ -1,9 +1,9 @@
-// Fused volumetric renderer, tensor-core decoder, RAY-PAIR variant (sm_100a). Same pipeline, bookkeeping and arithmetic as
+// Fused volumetric renderer, tensor-core decoder, RAY-PAIR variant (sm_90a). Same pipeline, bookkeeping and arithmetic as
 // render_tc.cu (reference training/volumetric_rendering/renderer.py:88-253, ray_marcher.py:25-57), different ownership:
-//   * a 128-thread group owns TWO WHOLE RAYS per iteration: ray A on tile rows / TMEM lanes 0..63, ray B on 64..127 (sample
+//   * a 128-thread group (one warpgroup) owns TWO WHOLE RAYS per iteration: ray A on tile rows 0..63, ray B on 64..127 (sample
 //     s of a ray on row 64 * ray + s, so Sc, Sf <= 64), coarse samples in one 128-row A-operand tile, fine samples in a
 //     second one;
-//   * nothing crosses a group: every synchronisation is the group's named barrier or its mbarrier, and the three groups
+//   * nothing crosses a group: every synchronisation is the group's named barrier, and the three groups
 //     of a CTA drift apart, so one group's texel gathers (bound by the SM's L2 ingest) overlap the other groups' decoder
 //     epilogues (bound by issue / XU) instead of all twelve warps hitting the same phase together as in render_tc.cu;
 //   * rows s >= Sc (Sf) of a half tile are dead: their lanes run predicated-off work (75 % lane use at 48 samples per
@@ -16,7 +16,7 @@ struct PairLayout {
     int Sc, Sf, S, gc, gf, NGc, NGf, cout;
     int ray_stride, o_dC, o_sC, o_dF, o_sF, o_sd, o_ss, o_w, o_cdf, o_om;
     int grp_bytes, g_feat, g_ray, g_part, g_scal;      // offsets inside a group's block
-    int off_tail, off_groups, off_bar, total_bytes;
+    int off_tail, off_groups, total_bytes;
 };
 
 __host__ __device__ inline PairLayout make_pair_layout(int Sc, int Sf, int n_nets) {
@@ -44,8 +44,6 @@ __host__ __device__ inline PairLayout make_pair_layout(int Sc, int Sf, int n_net
     int o = kTcTail;
     L.off_groups = o; o += 3 * L.grp_bytes;
     L.off_tail = o; o += kTcTailFloats * 4;
-    o = round_up(o, 8);
-    L.off_bar = o; o += 3 * 8 + 16;
     L.total_bytes = o;
     return L;
 }
@@ -58,7 +56,6 @@ struct PairParams {
 };
 
 constexpr int kPairThreads = 384;
-constexpr int kPairCols = 160;          // D1: [0,128)  D2: [128,160)
 
 __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(const PairParams P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -77,11 +74,9 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
     float* scal = reinterpret_cast<float*>(gb + L.g_scal);
     const float* tail = reinterpret_cast<const float*>(smem + L.off_tail);
     const float* b1 = tail, *b2c = tail + 128, *b2s = tail + 192, *w2s = tail + 196;
-    uint64_t* mma_bar = reinterpret_cast<uint64_t*>(smem + L.off_bar);
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(mma_bar + 3);
     __shared__ uint32_t cta_keys[2];
 
-    // ---- one-time setup: weights -> smem, dead rows zeroed, barriers, TMEM ------------------------------------------
+    // ---- one-time setup: weights -> smem, dead rows zeroed ------------------------------------------
     {
         const uint4* src = reinterpret_cast<const uint4*>(a.decoder_packed);
         uint4* dst = reinterpret_cast<uint4*>(smem);
@@ -92,64 +87,27 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
         uint4* z = reinterpret_cast<uint4*>(smem + L.off_groups);
         for (int i = tid; i < 3 * L.grp_bytes / 16; i += kPairThreads) z[i] = make_uint4(0u, 0u, 0u, 0u);
     }
-    if (tid == 0) {
-        for (int g = 0; g < 3; ++g) tc::mbar_init(&mma_bar[g], 1);
-        tc::fence_barrier_init();
-        cta_keys[0] = 0u; cta_keys[1] = 0u;
-    }
-    if (warp == 0) tc::tmem_alloc(tmem_ptr_smem, 512);
+    if (tid == 0) { cta_keys[0] = 0u; cta_keys[1] = 0u; }
     tc::fence_proxy_async();
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_grp = *tmem_ptr_smem + (uint32_t)(grp * kPairCols);
-    const uint32_t tmem_row = tmem_grp + ((uint32_t)(q * 32) << 16);
-    uint32_t bar_phase = 0;
     const uint32_t w1a = tc::smem_u32(smem + kTcW1A), w1b = tc::smem_u32(smem + kTcW1B);
-    const uint32_t idesc_n128 = tc::umma_idesc_f16(128, 128, 0), idesc_n64 = tc::umma_idesc_f16(128, 64, 0),
-                   idesc_n32 = tc::umma_idesc_f16(128, 32, 0);
     const int sig = a.sigma_net;
     const TcPlaneView pv{a.planes_nhwc, a.H, a.W, P.img_stride, P.plane_stride, P.pix_stride};
-
-    auto issue_layer1 = [&](int tile, int row0, uint32_t idesc) {
-        const uint32_t fa = tc::smem_u32(feat + tile * 16384);
-        const uint64_t da = tc::umma_desc_k128(fa);
-        const uint64_t dba = tc::umma_desc_k128(w1a + row0 * 128), dbb = tc::umma_desc_k128(w1b + row0 * 128);
+    auto group_sync = [&]() { tc::named_bar_sync(1 + grp, 128); };
+    // density of every row this thread owns a fragment of -> the ray buffer (row = 64 * ray of the pair + sample slot)
+    auto density = [&](int tile, int n, int o_s, int pair) {
+        DecHidden hd;
+        float sg[2][2];
+        dec_hidden<true>(tc::smem_u32(feat + tile * 16384), w1a, w1b, sig, b1, w2s, b2s, lane, hd, sg);
+        if ((lane & 3) == 0) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16(tmem_grp, da + 2 * k, dba + 2 * k, idesc, k != 0);
+            for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-        for (int k = 0; k < 2; ++k) tc::umma_f16(tmem_grp, da + 2 * k, dbb + 2 * k, idesc, 1);
-        tc::umma_commit(&mma_bar[grp]);
-    };
-    auto issue_layer2 = [&](int net) {
-        const uint32_t ahi = tmem_grp + net * 64, alo = ahi + 32, d2 = tmem_grp + 128;
-        const uint64_t bh = tc::umma_desc_k128(tc::smem_u32(smem + kTcW2H + net * 8192));
-        const uint64_t bl = tc::umma_desc_k128(tc::smem_u32(smem + kTcW2L + net * 8192));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, ahi + 8 * k, bh + 2 * k, idesc_n32, k != 0);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, alo + 8 * k, bh + 2 * k, idesc_n32, 1);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16_ts(d2, ahi + 8 * k, bl + 2 * k, idesc_n32, 1);
-        tc::umma_commit(&mma_bar[grp]);
-    };
-    auto group_sync = [&]() { tc::tc_fence_before(); tc::named_bar_sync(1 + grp, 128); tc::tc_fence_after(); };
-    auto wait_mma = [&]() { tc::mbar_wait(&mma_bar[grp], bar_phase); bar_phase ^= 1; tc::tc_fence_after(); };
-    auto sigma_from_tmem = [&]() -> float {
-        float acc0 = b2s[sig], acc1 = 0.f;
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-            uint32_t v[32];
-            tc::tmem_ld_32x32(tmem_row + hf * 32, v);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) {
-                const int jj = hf * 32 + j;
-                acc0 = fmaf(w2s[sig * 64 + jj], softplus2(__uint_as_float(v[j]) + b1[sig * 64 + jj]), acc0);
-                acc1 = fmaf(w2s[sig * 64 + jj + 1], softplus2(__uint_as_float(v[j + 1]) + b1[sig * 64 + jj + 1]), acc1);
-            }
+                for (int h = 0; h < 2; ++h) {
+                    const int s_r = dec_frag_row(mb, h, q, lane) & 63;
+                    if (pair * 2 + mb < P.total_rays && s_r < n) rayb[mb * L.ray_stride + o_s + s_r] = sg[mb][h];
+                }
         }
-        return acc0 + acc1;
     };
 
     for (int pair = blockIdx.x * 3 + grp; pair < P.n_pairs; pair += gridDim.x * 3) {
@@ -179,10 +137,8 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
             tc_gather_rows(pv, feat, q, lane, vC, b, px, py, pz);
             tc::fence_proxy_async();
             group_sync();
-            if (m == 0) issue_layer1(0, sig * 64, idesc_n64);
-            wait_mma();
-            const float sg = sigma_from_tmem();
-            if (vC) { rb[L.o_dC + sidx] = dC; rb[L.o_sC + sidx] = sg; }
+            density(0, Sc, L.o_sC, pair);
+            if (vC) rb[L.o_dC + sidx] = dC;
         }
         group_sync();
 
@@ -224,10 +180,8 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
             tc_gather_rows(pv, feat + 16384, q, lane, vF, b, px, py, pz);
             tc::fence_proxy_async();
             group_sync();
-            if (m == 0) issue_layer1(1, sig * 64, idesc_n64);
-            wait_mma();
-            const float sg = sigma_from_tmem();
-            if (vF) { rb[L.o_dF + sidx] = dF; rb[L.o_sF + sidx] = sg; }
+            density(1, Sf, L.o_sF, pair);
+            if (vF) rb[L.o_dF + sidx] = dF;
             group_sync();
         }
 
@@ -303,38 +257,24 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
                 const float wl = rank > 0 ? rb[L.o_w + rank - 1] : 0.f;
                 coef = 0.5f * (wl + rb[L.o_w + rank]);
             }
-            group_sync();      // every row of the group is done with D1 / D2 of the previous step
-            if (m == 0) issue_layer1(pass, 0, n_nets == 2 ? idesc_n128 : idesc_n64);
-            wait_mma();
-#pragma unroll 1
-            for (int net = 0; net < n_nets; ++net) {
-                uint32_t ph[32], pl[32];
+            // colour pre-activations of both nets from this pass's feature tile, then the tile is their staging area
+            float d2[2][2][16];
 #pragma unroll
-                for (int hf = 0; hf < 2; ++hf) {
-                    uint32_t vv[32];
-                    tc::tmem_ld_32x32(tmem_row + net * 64 + hf * 32, vv);
-                    tc::tmem_ld_wait();
+            for (int net = 0; net < 2; ++net) {
+                if (net >= n_nets) break;
+                DecHidden hd;
+                float sn[2][2];
+                dec_hidden<false>(tc::smem_u32(feat + pass * 16384), w1a, w1b, net, b1, w2s, b2s, lane, hd, sn);
+                dec_colours(hd, tc::smem_u32(smem + kTcW2H + net * 8192), tc::smem_u32(smem + kTcW2L + net * 8192), d2[net]);
+            }
+            group_sync();      // every warp's MMAs have read the feature tile
 #pragma unroll
-                    for (int j = 0; j < 32; j += 2) {
-                        const int jj = net * 64 + hf * 32 + j;
-                        const float h0 = softplus2(__uint_as_float(vv[j]) + b1[jj]);
-                        const float h1 = softplus2(__uint_as_float(vv[j + 1]) + b1[jj + 1]);
-                        const __half2 hh = __floats2half2_rn(h0, h1);
-                        const float2 back = __half22float2(hh);
-                        const __half2 ll = __floats2half2_rn(h0 - back.x, h1 - back.y);
-                        ph[hf * 16 + j / 2] = *reinterpret_cast<const uint32_t*>(&hh);
-                        pl[hf * 16 + j / 2] = *reinterpret_cast<const uint32_t*>(&ll);
-                    }
-                }
-                tc::tmem_st_32x32(tmem_row + net * 64, ph);
-                tc::tmem_st_32x32(tmem_row + net * 64 + 32, pl);
-                tc::tmem_st_wait();
+            for (int net = 0; net < 2; ++net) {
+                if (net >= n_nets) break;
+                dec_stage_rows(d2[net], feat + pass * 16384, q, lane);
                 group_sync();
-                if (m == 0) issue_layer2(net);
-                wait_mma();
                 uint32_t cv[32];
-                tc::tmem_ld_32x32(tmem_row + 128, cv);
-                tc::tmem_ld_wait();
+                dec_read_row(feat + pass * 16384, m, cv);
                 const uint32_t smask = a.sigmoid_mask[net];
                 float acc[32];
 #pragma unroll
@@ -371,6 +311,7 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
                             *reinterpret_cast<float4*>(dst + i) = make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
                     }
                 }
+                group_sync();  // the staging rows are rewritten by the next net
             }
         }
         group_sync();
@@ -394,12 +335,7 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
     // ---- global depth clamp (ray_marcher.py:49-50) ---------------------------------------------------------------
     __shared__ bool is_last;
     __threadfence();
-    tc::tc_fence_before();
     __syncthreads();
-    if (warp == 0) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(*tmem_ptr_smem, 512);
-    }
     if (tid == 0) {
         atomicMax(a.workspace + 0, cta_keys[0]);
         atomicMax(a.workspace + 1, cta_keys[1]);

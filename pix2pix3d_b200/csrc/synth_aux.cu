@@ -2,7 +2,7 @@
 // NCHW<->NHWC converters, the NHWC FIR + noise + bias + lrelu tail of an up=2 layer and the skip-image upsampler.
 // All are HBM-streaming kernels with 8/16-byte vector accesses along the (contiguous) channel axis.
 #include "p3d_common.cuh"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 #include "tmap.cuh"
 
 namespace p3d {
@@ -428,8 +428,8 @@ __global__ void __launch_bounds__(256) fir_act_nhwc_kernel(const __grid_constant
     }
 }
 
-// ---- packed fp32 pairs: sm_100 issues two IEEE fp32 operations per lane with FFMA2 / FADD2 / FMUL2 (PTX .f32x2). Each half
-// is rounded exactly as the scalar instruction would, so a kernel written on pairs is bit-identical to its scalar form.
+// ---- fp32 pairs: two IEEE fp32 operations on a packed pair (sm_90 has no paired fp32 instruction, so each half is one
+// scalar FFMA / FADD / FMUL, rounded exactly as written).
 __device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
     uint64_t r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -441,19 +441,16 @@ __device__ __forceinline__ float2 f2_unpack(uint64_t v) {
     return r;
 }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
+    const float2 x = f2_unpack(a), y = f2_unpack(b), z = f2_unpack(c);
+    return f2_pack(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
 }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    const float2 x = f2_unpack(a), y = f2_unpack(b);
+    return f2_pack(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y));
 }
 __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    const float2 x = f2_unpack(a), y = f2_unpack(b);
+    return f2_pack(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
 }
 
 // Separable form of the FIR tail for rank-1 filters f[j][i] = fy[j] * fx[i] (upfirdn2d.setup_filter([1,3,3,1]) is one: the

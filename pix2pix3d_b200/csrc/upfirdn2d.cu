@@ -1,4 +1,4 @@
-// upfirdn2d for sm_100a: pad -> zero-insert upsample -> FIR -> decimate, per (n, c) plane.
+// upfirdn2d for sm_90a: pad -> zero-insert upsample -> FIR -> decimate, per (n, c) plane.
 // Replaces torch_utils/ops/upfirdn2d.cu:33-379 + upfirdn2d.cpp:20-102 of the reference, plus a fused
 // FIR + demod + noise + bias + activation epilogue for the up=2 modulated-conv path
 // (training/networks_stylegan2.py:324-331, torch_utils/ops/conv2d_resample.py:128).

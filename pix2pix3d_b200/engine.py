@@ -2,7 +2,7 @@
 
 Executes `SynthesisBlock` / `SynthesisBlockNoUp` stacks (reference training/networks_stylegan2.py:419-463,
 training/superresolution.py:244-289) with NHWC fp16 activations: per-sample modulated weights
-(`p3d_modulate_weights`), tcgen05 implicit-GEMM convolutions (`p3d_conv_gemm`) with noise/bias/lrelu/clamp in the
+(`p3d_modulate_weights`), wgmma implicit-GEMM convolutions (`p3d_conv_gemm`) with noise/bias/lrelu/clamp in the
 epilogue, the four-phase stride-2 transposed convolution followed by one fused FIR+noise+bias+lrelu pass for up=2
 layers, and ToRGB accumulated straight into the upsampled fp32 skip image.
 
@@ -531,7 +531,7 @@ def encoder_forward(enc, img):
     for res in enc.block_resolutions:
         x = _encoder_block(getattr(enc, f'b{res}'), x, xin, b, res)
     # projector: a 4x4 "valid" convolution of the 4x4 map = one GEMM over (y, x, c); cuDNN picks an FFT algorithm for this
-    # shape (3.7 ms), a plain fp32 matmul against the NHWC-ordered weight streams the 117 MB of weights once
+    # shape, a plain fp32 matmul against the NHWC-ordered weight streams the 117 MB of weights once
     proj = enc.projector
     wp = _cached(proj, 'proj_nhwc', [proj.weight],
                  lambda: (proj.weight.detach().float().permute(0, 2, 3, 1).reshape(proj.weight.shape[0], -1) * proj.scale).contiguous())

@@ -2,7 +2,7 @@
 
 One `G.synthesis` is ~250 kernel launches (libp3d.so kernels plus a few small ATen ops: affine layers, RNG draws,
 casts). Captured once into a CUDA graph, a step becomes a single graph launch, so the host is off the critical
-path -- the B200-side replacement for what a tracing compiler would be used for. Random draws inside the capture
+path -- the GPU-side replacement for what a tracing compiler would be used for. Random draws inside the capture
 (stratified jitter, importance u) use torch's graph-safe Philox generator, so every replay draws fresh numbers.
 """
 import torch

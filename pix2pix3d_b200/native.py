@@ -237,8 +237,8 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
     use_tc = impl in ('auto', 'tc', 'tc_pairs') and Sc % 8 == 0 and Sf % 8 == 0 and Sc <= 128 and Sf <= 128 and dec.packed_tc is not None
     if impl in ('tc', 'tc_pairs') and not use_tc:
         raise ValueError('tensor-core renderer needs sample counts that are multiples of 8')
-    # ray-pair ownership fills its rows only at 64 samples per pass; there it is 6-8 % faster (1.58 vs 1.72 ms at the config-4
-    # sampling), at 48 it is 21 % slower (profiles/r01_render_fwd_tc_ncu.md)
+    # ray-pair ownership fills its 64-row halves only at 64 samples per pass; at fewer samples per ray the row-tiled kernel
+    # packs its tiles densely and the pair kernel would leave rows idle
     a.tc_variant = 1 if (impl == 'tc_pairs' or (impl == 'auto' and Sc == 64 and Sf == 64)) else 0
     with torch.cuda.device(dev):
         if use_tc:

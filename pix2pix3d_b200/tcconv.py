@@ -38,12 +38,6 @@ class ConvArgs(ctypes.Structure):  # p3d_conv_args_t
     ]
 
 
-# A/B switches of the convolution launcher (p3d_conv_args_t::launch_flags; results do not depend on them): bit 0 = never the
-# persistent kernel, bit 1 = never CTA pairs. The environment is read HERE, once, by the host binding -- the library has no
-# process-global switches.
-launch_flags = (1 if os.environ.get('P3D_CONV_PERSIST') == '0' else 0) | (2 if os.environ.get('P3D_CONV_PAIR') == '0' else 0)
-
-
 def pad_to(n, m):
     return (n + m - 1) // m * m
 
@@ -201,7 +195,6 @@ def _conv_args(x, w, cout, taps, grid_hw, out, out_lo=None, out_mode=0, out_map=
         assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
     a.act, a.alpha, a.gain, a.clamp, a.acc_scale = act, alpha, gain, clamp, acc_scale
     a.stride = stride
-    a.launch_flags = launch_flags
     if residual is not None:
         assert residual.dtype == torch.float32 and residual.is_contiguous() and tuple(residual.shape) == (b, grid_hw[0], grid_hw[1], cout)
         a.residual = residual.data_ptr()

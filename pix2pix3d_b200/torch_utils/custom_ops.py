@@ -4,8 +4,9 @@ The reference JIT-compiles a pybind module per op on first use and hands it to `
 classes call `_plugin.bias_act(...)`, `_plugin.upfirdn2d(...)`, `_plugin.filtered_lrelu(...)`,
 `_plugin.filtered_lrelu_act_(...)` (bias_act.cpp:36, upfirdn2d.cpp:20, filtered_lrelu.cpp:20,217). Here the plugins are
 ahead-of-time objects over libp3d.so's C-ABI (include/p3d.h) with those very call signatures, so the REFERENCE's own
-`torch_utils/ops/{bias_act,upfirdn2d,filtered_lrelu}.py` run unmodified on the sm_100a kernels when this module stands in
-for the reference's (`tests/test_gpu_plugins.py` does exactly that). Nothing is compiled at import or call time;
+`torch_utils/ops/{bias_act,upfirdn2d,filtered_lrelu}.py` run unmodified on the sm_90a kernels when this module stands in
+for the reference's (`tests/test_gpu_vs_reference.py::test_reference_op_wrappers_run_on_libp3d_plugins` and
+`::test_reference_filtered_lrelu_wrapper_runs_on_libp3d_plugin` do exactly that). Nothing is compiled at import or call time;
 `sources`, `headers`, `source_dir` and build kwargs are accepted and ignored.
 """
 import torch

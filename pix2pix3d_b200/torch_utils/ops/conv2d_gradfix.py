@@ -3,7 +3,7 @@
 Surface of the reference's torch_utils/ops/conv2d_gradfix.py (:23 `enabled`, :26-33 `no_weight_gradients`,
 :37-45 entry points). The forward / data-gradient / weight-gradient convolutions are ATen calls, exactly as in the reference
 (:128-129, :169) -- except inside `native_conv.first_order()` regions (the generator's training passes), where fp32 stride-1
-convolutions run forward and input gradient on libp3d's tcgen05 implicit GEMM (native_conv.py). The inference path does not go
+convolutions run forward and input gradient on libp3d's wgmma implicit GEMM (native_conv.py). The inference path does not go
 through this module (engine.py drives the same kernels directly).
 """
 import contextlib

@@ -1,7 +1,7 @@
 """Filtered leaky ReLU: bias -> upsample FIR -> lrelu(gain, slope, clamp) -> downsample FIR.
 
 Surface of the reference's torch_utils/ops/filtered_lrelu.py:58 `filtered_lrelu` (only caller: StyleGAN3's alias-free
-synthesis layer, training/networks_stylegan3.py:357). CUDA tensors run the fused sm_100a kernel `p3d_filtered_lrelu`
+synthesis layer, training/networks_stylegan3.py:357). CUDA tensors run the fused sm_90a kernel `p3d_filtered_lrelu`
 (csrc/filtered_lrelu.cu: the up-sampled intermediate stays in shared memory); its gradient is the same kernel with the
 filters swapped and flipped, steered by the 2-bit sign tensor the forward pass wrote (reference :155-274). Configurations
 the kernel reports as unsupported (the reference's `rc = -1`) compose `upfirdn2d` + the in-place sign-aware activation

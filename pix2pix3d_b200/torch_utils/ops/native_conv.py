@@ -1,6 +1,6 @@
-"""fp32 convolutions of the training path on the tcgen05 implicit-GEMM kernel (`p3d_conv_gemm`, three-pass fp16 split = fp32
-accuracy) instead of cuDNN's fp32 SIMT kernels (TF32 is off during training, training_loop.py:278-279, which leaves cuDNN at
-~60 TFLOP/s on a B200).
+"""fp32 convolutions of the training path on the wgmma implicit-GEMM kernel (`p3d_conv_gemm`, three-pass fp16 split = fp32
+accuracy) instead of cuDNN's fp32 SIMT kernels (TF32 is off during training, training_loop.py:278-279, which leaves cuDNN on
+its fp32 CUDA-core kernels).
 
 Scope: what `conv2d_gradfix.conv2d` receives from the non-fused modulated convolutions of the generator and from the label-map
 Encoder when gradients are required (`networks_stylegan2.py:68-75`, `conv2d_resample.py:134-136`): 3x3 (padding 1) and 1x1
@@ -9,7 +9,7 @@ up=2 layers (`conv2d_resample.py:114-128`: 3x3, stride 2, padding 0 -> the (2H+1
 the input gradient run on libp3d (the input gradient of a stride-1 convolution is the same convolution with the kernel flipped
 and its channel axes swapped; the transposed convolution runs as its four phase GEMMs in one launch, its input gradient is a
 stride-2 'valid' convolution of the incoming gradient with the same weight tensor); the weight
-gradient stays ATen's `convolution_backward` (a tcgen05 wgrad needs MN-major operand tiles: not built). First-order only: the
+gradient stays ATen's `convolution_backward` (a tensor-core wgrad needs MN-major operand tiles: not built). First-order only: the
 node is used where no double backward can follow (inside `first_order()`, which the generator's `mapping` / `synthesis` /
 `sample_mixed` enter; the discriminators, whose R1 penalty differentiates twice, never do).
 """

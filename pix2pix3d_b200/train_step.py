@@ -12,7 +12,7 @@ Every network / op class is resolved through the reference's import paths (`trai
   * product arm: `pix2pix3d_b200.install(reference_root=...)` is active, so G, D, the ops and kernels are this package's
     and only the host-side loss class comes from the reference checkout (the drop-in scenario of BASELINE.json.north_star:
     "train.py calls into it unchanged");
-  * reference arm: nothing is installed and everything resolves to the unmodified reference (baseline/_ref).
+  * reference arm: nothing is installed and everything resolves to the unmodified reference (a verbatim copy, oracle/_ref).
 `lpips` (training/loss.py:20, a VGG download) is not available offline: a stub returning zeros is injected and the
 configuration sets lambda_lpips = 0, as SURVEY.md 8c prescribes; G / D / R1 arithmetic is unaffected.
 """

@@ -2,7 +2,7 @@
 
 Mirror of the reference's training/dual_discriminator.py (`filtered_resizing` :86-102, `DualDiscriminator` :107-172,
 `SingleDiscriminator` :21-80, `DummyDualDiscriminator` :179-245). Built from the same DiscriminatorBlock / Epilogue modules, whose FIR and bias_act work
-runs on the sm_100a kernels; the convolutions go through `conv2d_gradfix`. Only needed by BASELINE config 5 (train step).
+runs on the sm_90a kernels; the convolutions go through `conv2d_gradfix`. Only needed by BASELINE config 5 (train step).
 """
 import numpy as np
 import torch

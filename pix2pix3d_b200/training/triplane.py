@@ -153,7 +153,7 @@ class TriPlaneGenerator(torch.nn.Module):
 def mark_first_order(*classes):
     """The generator is differentiated once per pass in every loss of the reference (training/loss.py: no path-length or other
     second-order term touches G): run its `mapping` / `synthesis` / `sample` / `sample_mixed` inside
-    `native_conv.first_order()`, which lets the fp32 training convolutions use the tcgen05 implicit GEMM for forward and input
+    `native_conv.first_order()`, which lets the fp32 training convolutions use the wgmma implicit GEMM for forward and input
     gradient (torch_utils/ops/native_conv.py). The discriminators never enter such a region (R1 differentiates twice)."""
     import functools
     from ..torch_utils.ops import native_conv

@@ -2,7 +2,7 @@
 torch_utils/persistence.py:181-204) as mirror classes and reproduce the reference's outputs.
 
 The pickle is produced at test time by the reference itself in a subprocess (it embeds the reference's module sources, so it
-is never committed); the test is skipped where the reference checkout does not exist (the GPU box)."""
+is never committed); it reads the reference from the copy build() makes in oracle/_ref (oracle/vendor_reference.py)."""
 import io
 import os
 import subprocess
@@ -16,8 +16,8 @@ import torch
 from conftest import load_golden, rel_err
 from make_golden import SYNTH_CASES
 
-REF = '/root/reference'
 ORACLE_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', 'oracle')
+REF = os.path.abspath(os.path.join(ORACLE_DIR, '_ref'))
 
 WRITER = textwrap.dedent('''
     import pickle, sys
@@ -37,9 +37,20 @@ WRITER = textwrap.dedent('''
 ''')
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason='needs the reference checkout to write the pickle')
+@pytest.fixture
+def install():
+    """pix2pix3d_b200.install() for one test: the aliases are removed again afterwards, so that later tests in the process can
+    import the reference's own modules under the same names."""
+    import pix2pix3d_b200
+    try:
+        yield pix2pix3d_b200.install
+    finally:
+        pix2pix3d_b200.uninstall()
+
+
+@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, 'training')), reason='needs the reference copy build() makes in oracle/_ref')
 @pytest.mark.parametrize('case_name', ['seg_tiny', 'rgb_tiny'])
-def test_reference_pickle_loads_as_mirror_classes(tmp_path, case_name):
+def test_reference_pickle_loads_as_mirror_classes(tmp_path, case_name, install):
     pkl = str(tmp_path / 'network.pkl')
     code = WRITER.format(ref=REF, oracle=os.path.abspath(ORACLE_DIR), case=case_name, out=pkl)
     r = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, timeout=600)
@@ -49,8 +60,7 @@ def test_reference_pickle_loads_as_mirror_classes(tmp_path, case_name):
     assert b'_reconstruct_persistent_obj' in raw and b'class SynthesisLayer' in raw      # reference format: embedded source
 
     # the reference's calling sequence (generate_samples.py:93-95) through the aliased import paths
-    import pix2pix3d_b200
-    pix2pix3d_b200.install()
+    install()
     import dnnlib
     import legacy
     with dnnlib.util.open_url(pkl) as f:

@@ -63,7 +63,7 @@ def test_decoder_mlp_many_tiles_against_float64(monkeypatch):
     dec = tc.OSGDecoder_semantic_entangle(32, {'decoder_lr_mul': 1.0, 'decoder_output_dim': 32, 'sigmoid': False, 'semantic_channels': 6}).cuda()
     for p in dec.parameters():
         p.data.normal_(0, 1.0)
-    n, m = 3, 148 * 128 * 2 // 3 + 5
+    n, m = 3, 132 * 128 * 2 // 3 + 5
     feats = (torch.randn(n, 3, m, 32, device='cuda') * 6).requires_grad_(True)
     params = list(dec.parameters())
     out = dec(feats, None)

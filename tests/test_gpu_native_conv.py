@@ -1,4 +1,4 @@
-"""fp32 training convolutions on the tcgen05 implicit GEMM (torch_utils/ops/native_conv.py): forward and both gradients against
+"""fp32 training convolutions on the wgmma implicit GEMM (torch_utils/ops/native_conv.py): forward and both gradients against
 fp64 ATen convolutions; dispatch rules of conv2d_gradfix (only inside first_order() regions, only the shapes the node covers)."""
 import pytest
 import torch

@@ -142,7 +142,7 @@ def test_split_k_small_grids_match_single_pass_order():
     ref = F.conv2d(x.double().cpu(), wt.double().cpu(), padding=1) + noise.double().cpu() + bias.double().cpu()[None, :, None, None]
     ref = F.leaky_relu(ref, 0.2) * np.sqrt(2)
     for o in outs:
-        assert rel_err(o.permute(0, 3, 1, 2).cpu().numpy(), ref.numpy()) < 3e-5      # K = 4608: fp32 TMEM accumulation
+        assert rel_err(o.permute(0, 3, 1, 2).cpu().numpy(), ref.numpy()) < 3e-5      # K = 4608: fp32 accumulation
     # the two orders differ by the tensor core's truncating fp32 accumulation over K = 4608 (split-K rounds partials properly)
     assert rel_err(outs[1].cpu().numpy(), outs[0].cpu().numpy()) < 4e-5
 
@@ -275,12 +275,12 @@ def test_fused_torgb_tail_matches_upsample_plus_conv(cout, hw, split, nchw):
 
 
 @pytest.mark.parametrize('split', [False, True])
-def test_cta_pair_kernel_256_channel_tiles(split):
-    """Layers with >= 256 output channels and >= 74 tile pairs run on CTA pairs (cta_group::2, one 256x256 tile per two
-    SMs); the result must equal the single-CTA kernels' (P3D_CONV_PAIR=0 is read once per process, so compare with torch)."""
+def test_wide_layer_512_channels(split):
+    """A 512-channel 3x3 layer over a few hundred tiles (four 128-channel tiles per pixel tile, odd tile edges), against
+    torch."""
     from pix2pix3d_b200 import tcconv
     torch.manual_seed(21)
-    b, c, h, w, cout = 2, 128, 96, 80, 512           # 2 * ceil(96*80/256) * 2 = 120 tile pairs, odd tile edges
+    b, c, h, w, cout = 2, 128, 96, 80, 512           # 2 * ceil(96*80/128) * 4 = 480 tiles, odd tile edges
     x = torch.randn(b, c, h, w, device='cuda')
     wt = torch.randn(cout, c, 3, 3, device='cuda') / np.sqrt(9 * c)
     bias = torch.randn(cout, device='cuda')
@@ -303,7 +303,7 @@ def test_cta_pair_kernel_256_channel_tiles(split):
 
 def test_strided_conv_and_residual_epilogue():
     """down=2 layers: out(y, x) = sum_d w[d] * in(2y + dy, 2x + dx) through TMA element strides, plus the resnet skip tensor
-    added after the activation; small (split-K-sized) and large (persistent / pair kernel) shapes."""
+    added after the activation; small (split-K-sized) and large (many tiles, 256 channels) shapes."""
     from pix2pix3d_b200 import tcconv
     torch.manual_seed(14)
     for b, c, hw, cout in ((2, 64, 17, 64), (2, 128, 129, 128), (1, 64, 257, 256)):
@@ -344,8 +344,8 @@ def test_strided_conv_and_residual_epilogue():
     (2, 64, 48, (7, 5), False),          # grid kernel, no split-K (Cin 64: 4 k-steps in the heaviest phase)
     (4, 512, 512, (4, 4), True),         # grid kernel + split-K partials per phase + one finisher for all phases
     (4, 512, 512, (16, 16), True),       # the b32 up layer: grid kernel, split-K
-    (2, 128, 128, (72, 64), False),      # persistent kernel (one tile schedule over the four phases)
-    (1, 256, 256, (56, 72), True),       # CTA-pair kernel, three-pass split
+    (2, 128, 128, (72, 64), False),      # many tiles: one tile range per phase in the launch
+    (1, 256, 256, (56, 72), True),       # two channel tiles, three-pass split
 ])
 def test_merged_transposed_conv_phases_equal_separate_launches(b, c, cout, hw, split, monkeypatch):
     """p3d_conv_gemm_phases: one launch over the four phases == four p3d_conv_gemm launches, bit for bit, and both match the
@@ -367,8 +367,8 @@ def test_merged_transposed_conv_phases_equal_separate_launches(b, c, cout, hw, s
         assert torch.isfinite(out).all(), 'every output pixel must be written by exactly one phase'
         outs.append(out)
     if split:
-        # fp32 accumulators: the merged launch may pick another kernel shape (CTA pairs: M = 256 MMAs) or another split-K factor than
-        # the separate launches do -> another summation grouping, equal to rounding
+        # fp32 accumulators: the merged launch may pick another split-K factor than the separate launches do -> another summation
+        # grouping, equal to rounding
         assert torch.allclose(outs[0], outs[1], rtol=0, atol=1e-5 * float(outs[1].abs().max()))
     else:
         assert torch.equal(outs[0], outs[1])
@@ -395,10 +395,11 @@ def test_conv_gemm_phases_rejects_mismatched_phases():
     assert _lib.lib().p3d_conv_gemm_phases(arr, 5, _lib.stream_ptr()) == -2
 
 
-@pytest.mark.parametrize('cout,ci,hw,b', [(128, 3, (256, 256), 2), (128, 6, (192, 256), 2), (64, 3, (256, 256), 3)])
+@pytest.mark.parametrize('cout,ci,hw,b', [(128, 3, (256, 256), 2), (128, 6, (192, 256), 2), (64, 3, (256, 256), 3), (96, 3, (128, 128), 2)])
 def test_torgb_fused_into_the_producing_convolution(cout, ci, hw, b):
     """p3d_conv_args_t::rgb_*: the 3x3 convolution of the last super-resolution block also evaluates the block's ToRGB + skip
-    (networks_stylegan2.py:452-458) on the outputs it holds -- against the two separate launches it replaces."""
+    (networks_stylegan2.py:452-458) on the outputs it holds -- against the two separate launches it replaces. 96 channels run in
+    a 128-channel tile whose last 32 channels lie past Cout."""
     from pix2pix3d_b200 import tcconv
     from pix2pix3d_b200.torch_utils.ops import upfirdn2d
     torch.manual_seed(31)
@@ -413,13 +414,20 @@ def test_torgb_fused_into_the_producing_convolution(cout, ci, hw, b):
     prev = torch.randn(b, h // 2, w // 2, ci, device='cuda')
     xn = tcconv.to_nhwc_f16(x)
     wk = _weights_kmajor(w3, scale=tcconv.WEIGHT_SCALE)
-    wk_rgb = tcconv.modulate_weights(wrgb, styles, demodulate=False, pre_scale=0.7)       # [1,B,16,cout]: per-sample ToRGB weights
+    wk_rgb = tcconv.modulate_weights(wrgb, styles, demodulate=False, pre_scale=0.7, cin_padded=cout)   # [1,B,16,cout]: per-sample ToRGB weights
     # separate launches: conv -> fp16 x, then the fused-tail ToRGB convolution on it
     y = torch.empty(1, b, h, w, cout, device='cuda', dtype=torch.float16)
     tcconv.conv_gemm(xn, wk, cout, tcconv.TAPS_3X3, (h, w), y[0], out_mode=0, bias=bias3, act=3, alpha=0.2, gain=float(np.sqrt(2)), clamp=256.0)
-    ref = torch.empty(b, ci, h, w, device='cuda')
-    tcconv.conv_gemm(y, wk_rgb, ci, tcconv.TAPS_1X1, (h, w), ref, out_mode=2, bias=brgb, act=1, gain=1.0, clamp=256.0, up_prev=prev,
-                     up_filter=f, round16=True, out_nchw=True)
+    if cout % 64 == 0:
+        ref = torch.empty(b, ci, h, w, device='cuda')
+        tcconv.conv_gemm(y, wk_rgb, ci, tcconv.TAPS_1X1, (h, w), ref, out_mode=2, bias=brgb, act=1, gain=1.0, clamp=256.0, up_prev=prev,
+                         up_filter=f, round16=True, out_nchw=True)
+    else:
+        # a convolution reads its input in 64-channel k-steps, so no separate ToRGB launch takes 96 channels: the same
+        # arithmetic in torch (fp16 x and weights, dot x 1/WEIGHT_SCALE + bias, clamp, one fp16 rounding, + upsampled skip)
+        dot = torch.einsum('bhwk,bck->bchw', y[0].double(), wk_rgb[0, :, :ci].double()).float()
+        rgb = (dot / tcconv.WEIGHT_SCALE + brgb[None, :, None, None]).clamp(-256, 256).half().float()
+        ref = upfirdn2d.upsample2d(prev.permute(0, 3, 1, 2).contiguous(), f) + rgb
     for skip_x in (False, True):
         y2 = torch.full_like(y, float('nan'))
         out = torch.full((b, ci, h, w), float('nan'), device='cuda')
@@ -438,10 +446,12 @@ def test_torgb_fused_into_the_producing_convolution(cout, ci, hw, b):
 
 
 def test_torgb_fusion_is_refused_for_other_launch_shapes():
+    """The fused ToRGB needs every output channel of a pixel in one channel tile of at most 128 channels: a 192-channel
+    layer spans two tiles and is refused."""
     from pix2pix3d_b200 import tcconv
     from pix2pix3d_b200.torch_utils.ops import upfirdn2d
     f = upfirdn2d.setup_filter([1, 3, 3, 1]).cuda()
-    b, c, cout, ci, h = 1, 64, 64, 3, 16            # 1 tile: not the persistent kernel
+    b, c, cout, ci, h = 1, 64, 192, 3, 16
     xn = tcconv.to_nhwc_f16(torch.randn(b, c, h, h, device='cuda'))
     wk = _weights_kmajor(torch.randn(cout, c, 3, 3, device='cuda'))
     wk_rgb = _weights_kmajor(torch.randn(ci, cout, 1, 1, device='cuda'))

@@ -1,5 +1,5 @@
 """Every module of the package (and the repo-root entry points) imports on a machine without a GPU: a missing import in a module
-the CPU suite does not otherwise touch (engine.py, graphs.py, train_step.py ...) would only show up on the GPU box."""
+the CPU suite does not otherwise touch (engine.py, graphs.py, train_step.py ...) would only show up on a GPU machine."""
 import importlib
 import os
 import pkgutil

@@ -10,7 +10,9 @@ import textwrap
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = next((p for p in ('/root/reference', os.path.join(ROOT, 'baseline', '_ref')) if os.path.isdir(os.path.join(p, 'training'))), None)
+# the reference (pix2pix3D): the copy build() makes in oracle/_ref (oracle/vendor_reference.py), or $P3D_REFERENCE_ROOT
+REF = next((p for p in (os.path.join(ROOT, 'oracle', '_ref'), os.environ.get('P3D_REFERENCE_ROOT', ''))
+            if p and os.path.isdir(os.path.join(p, 'training'))), None)
 
 SCRIPT = textwrap.dedent('''
     import sys, types
@@ -67,7 +69,7 @@ SCRIPT = textwrap.dedent('''
 ''')
 
 
-@pytest.mark.skipif(REF is None, reason='needs a reference checkout (/root/reference or baseline/_ref)')
+@pytest.mark.skipif(REF is None, reason='needs the reference copy build() makes in oracle/_ref')
 @pytest.mark.parametrize('explicit', [True, False])
 def test_reference_callers_import_with_install_active(explicit):
     code = SCRIPT.format(root=ROOT, oracle=os.path.join(ROOT, 'oracle'), ref=REF,

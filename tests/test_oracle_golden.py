@@ -1,5 +1,5 @@
 """The oracle (oracle/p3d_oracle, numpy) against fixtures produced by the REFERENCE implementation
-(oracle/make_golden.py, run in the authoring container). This is what pins the oracle."""
+(oracle/make_golden.py, run against a reference checkout). This is what pins the oracle."""
 import numpy as np
 import pytest
 import torch

@@ -11,7 +11,9 @@ import textwrap
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = next((p for p in ('/root/reference', os.path.join(ROOT, 'baseline', '_ref')) if os.path.isdir(os.path.join(p, 'training'))), None)
+# the reference (pix2pix3D): the copy build() makes in oracle/_ref (oracle/vendor_reference.py), or $P3D_REFERENCE_ROOT
+REF = next((p for p in (os.path.join(ROOT, 'oracle', '_ref'), os.environ.get('P3D_REFERENCE_ROOT', ''))
+            if p and os.path.isdir(os.path.join(p, 'training'))), None)
 
 ARM = textwrap.dedent('''
     import json, sys
@@ -50,7 +52,7 @@ def _finish(p):
     return json.loads(line[7:])
 
 
-@pytest.mark.skipif(REF is None, reason='needs a reference checkout (/root/reference or baseline/_ref)')
+@pytest.mark.skipif(REF is None, reason='needs the reference copy build() makes in oracle/_ref')
 def test_training_iteration_matches_reference_on_cpu():
     procs = _start(False), _start(True)                      # the two arms run side by side (4 torch threads each)
     ref, ours = _finish(procs[0]), _finish(procs[1])

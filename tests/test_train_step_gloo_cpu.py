@@ -12,7 +12,9 @@ import textwrap
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = next((p for p in ('/root/reference', os.path.join(ROOT, 'baseline', '_ref')) if os.path.isdir(os.path.join(p, 'training'))), None)
+# the reference (pix2pix3D): the copy build() makes in oracle/_ref (oracle/vendor_reference.py), or $P3D_REFERENCE_ROOT
+REF = next((p for p in (os.path.join(ROOT, 'oracle', '_ref'), os.environ.get('P3D_REFERENCE_ROOT', ''))
+            if p and os.path.isdir(os.path.join(p, 'training'))), None)
 
 RANK = textwrap.dedent('''
     import json, os, sys
@@ -57,7 +59,7 @@ def _finish(p):
     return json.loads([ln for ln in out.splitlines() if ln.startswith('DIGEST ')][-1][7:])
 
 
-@pytest.mark.skipif(REF is None, reason='needs a reference checkout (/root/reference or baseline/_ref)')
+@pytest.mark.skipif(REF is None, reason='needs the reference copy build() makes in oracle/_ref')
 def test_two_gloo_ranks_end_the_iteration_with_identical_parameters():
     port = _free_port()
     procs = [_start(2, 0, port), _start(2, 1, port), _start(1, 0, port)]        # two ranks + a single-rank step on rank 0's shard

@@ -1,7 +1,7 @@
-"""Summarise an `ncu --set full` capture of one kernel: per-launch DRAM traffic (for bench.py's `roofline.traffic`) and the
-counters DESIGN.md quotes. Run where `ncu` exists (this container reads the .ncu-rep the GPU box wrote).
+"""Summarise an `ncu --set full` capture of one kernel: per-launch DRAM traffic and the
+main pipe / stall counters. Run where `ncu` can read the .ncu-rep.
 
-usage: python tools/ncu_traffic.py <report.ncu-rep> <kernel-substring> <workload> <batch> [out.json=profiles/render_traffic.json]
+usage: python tools/ncu_traffic.py <report.ncu-rep> <kernel-substring> <workload> <batch> [out.json=render_traffic.json]
 Writes/updates the JSON (one entry per workload/batch) and prints a markdown table of the main counters.
 """
 import csv
@@ -16,7 +16,7 @@ WANT = [
     'l1tex__t_sector_hit_rate.pct', 'sm__inst_executed.sum', 'sm__issue_active.avg.pct_of_peak_sustained_active',
     'sm__inst_executed_pipe_xu.avg.pct_of_peak_sustained_active', 'sm__inst_executed_pipe_alu.avg.pct_of_peak_sustained_active',
     'sm__inst_executed_pipe_fma.avg.pct_of_peak_sustained_active', 'sm__inst_executed_pipe_lsu.avg.pct_of_peak_sustained_active',
-    'sm__pipe_tensor_subpipe_umma_cycles_active.avg.pct_of_peak_sustained_active', 'sm__inst_executed_pipe_tensor.sum',
+    'sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active', 'sm__inst_executed_pipe_tensor.sum',
     'sm__warps_active.avg.pct_of_peak_sustained_active', 'launch__registers_per_thread', 'launch__shared_mem_per_block_dynamic',
     'l1tex__data_bank_conflicts_pipe_lsu_mem_shared.sum', 'smsp__pcsamp_warps_issue_stalled_long_scoreboard',
     'smsp__pcsamp_warps_issue_stalled_wait', 'smsp__pcsamp_warps_issue_stalled_mio_throttle', 'smsp__pcsamp_warps_issue_stalled_short_scoreboard',
@@ -36,8 +36,7 @@ def raw_rows(rep):
 
 def main():
     rep, kern, workload, batch = sys.argv[1], sys.argv[2], sys.argv[3], int(sys.argv[4])
-    out_path = sys.argv[5] if len(sys.argv) > 5 else os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                                                                  'profiles', 'render_traffic.json')
+    out_path = sys.argv[5] if len(sys.argv) > 5 else 'render_traffic.json'
     hdr, units, rows = raw_rows(rep)
     ik = hdr.index('Kernel Name')
     rows = [r for r in rows if kern in r[ik]]
