@@ -2,7 +2,7 @@
 // convolutions of the synthesis and super-resolution blocks (reference: training/networks_stylegan2.py:34-91,
 // torch_utils/ops/conv2d_resample.py:48-143, which bottom out in cuDNN).
 //
-//   D[128 pixels x BN channels] (registers of two warpgroups, fp32) += A[128 x 64] (smem) * B[BN x 64]^T (smem), fp16 operands
+//   D[128 pixels x BN channels] (registers of one warpgroup, fp32) += A[128 x 64] (smem) * B[BN x 64]^T (smem), fp16 operands
 //
 // * Activations are NHWC fp16, so the im2col operand of one filter tap is a plain 4-D TMA box
 //   {64 channels, BW, BH, 1 image} shifted by the tap offset; out-of-bounds coordinates are zero-filled by the
@@ -11,8 +11,9 @@
 //   [B][Cout][taps*Cin] fp16.
 // * fp32 layers (the tri-plane backbone) run as three fp16 passes over split operands, x = hi + lo,
 //   hi*hi + hi*lo + lo*hi, accumulated in the same fp32 accumulators (error ~2^-22, products are exact in fp32).
-// * Warp roles: warp 8 = TMA producer, warps 0-7 = two consumer warpgroups (wgmma, then the epilogue:
-//   scale/noise/bias/activation/clamp -> NHWC store). mbarrier ring of smem stages.
+// * Persistent ping-pong: warpgroup 0 = TMA producer, warpgroups 1 and 2 = consumers that own alternate tiles (wgmma, then
+//   the epilogue: scale/noise/bias/activation/clamp -> NHWC store), so one tile's epilogue runs under the next tile's MMAs.
+//   mbarrier ring of smem stages shared by the consumers.
 // * A launch may carry up to four PHASES (ConvPhase: tap subset, grid, output offset): the four parities of a stride-2
 //   transposed 3x3 convolution run as one launch (p3d_conv_gemm_phases).
 // * The kernel can also evaluate the NEXT layer's 1x1 ToRGB + skip on the outputs it holds (rgb_* arguments): the last
@@ -25,10 +26,11 @@
 
 namespace p3d {
 
-constexpr int kBM = 128;        // pixels per tile (two warpgroups of 64 rows)
+constexpr int kBM = 128;        // pixels per tile (two m64 wgmma row blocks)
 constexpr int kBK = 64;         // fp16 elements per k-step (128-byte swizzle span)
 constexpr int kMaxGroups = 27;  // 9 taps x 3 precision passes
 constexpr int kMaxStages = 6;   // deepest smem ring
+constexpr size_t kSmemPerBlock = 227 * 1024;     // sm_90 opt-in shared memory per block
 
 // One output phase of a launch. An ordinary convolution has one; a stride-2 transposed convolution run as ONE launch has four
 // (tap subsets of the same weight tensor over the same input, each writing its own parity of the (2H+1) x (2W+1) grid).
@@ -49,6 +51,7 @@ struct ConvKernelArgs {
     int Cin;
     // tiling
     int BW, BH, BN, w_per_sample;
+    int B, tiles_m, tiles_n, n_units;  // samples; spatial tiles (all phases) and channel tiles; work units = tiles x B x splits
     // epilogue
     int oH, oW, sy, sx;               // output tensor size and the stride of the output map (Y = y*sy + phase.oy)
     int Cout, y_cstride, y_coff;      // valid channels, channel stride of the output tensor, channel offset
@@ -58,7 +61,7 @@ struct ConvKernelArgs {
     int64_t noise_bstride;            // elements between the noise images of consecutive samples (0: one image for the batch)
     float alpha, clamp, acc_scale;
     int base_aligned;                 // y / y_lo are 32-byte aligned (256-bit stores allowed)
-    int splits;                       // split-K: blockIdx.z = b * splits + s; s covers k-steps [s*total/splits, (s+1)*total/splits)
+    int splits;                       // split-K: work unit sample index b * splits + s; s covers k-steps [s*total/splits, (s+1)*total/splits)
     float* partial;                   // split-K: raw fp32 accumulators, per phase [splits][B][gH][gW][Cout_pad] (finished by a second kernel)
     int Cout_pad;
     // fused ToRGB tail (SynthesisBlock.forward, networks_stylegan2.py:452-458): out = upsample2d(prev, f) + [fp16-rounded] y
@@ -262,223 +265,279 @@ __device__ __forceinline__ void conv_store_chunk(const ConvKernelArgs& a, uint32
                 }
 }
 
-// Warp roles: warps 0-7 = two consumer warpgroups (wgmma on tile rows 0-63 and 64-127, then the epilogue), warp 8 = TMA
-// producer. After the k-loop the accumulators are parked in the (then idle) stage ring as an fp32 [128 pixels][BN] tile so
-// that an epilogue thread owns one pixel and reads 32 consecutive channels, the form conv_store_chunk takes.
-constexpr int kConvThreads = 288;
+// Persistent, warp-specialised ping-pong kernel. Warpgroup 0 is the TMA producer (one thread); warpgroups 1 and 2 are
+// consumers. A CTA walks the work units (phase tile, channel tile, sample, k-split) blockIdx.x, blockIdx.x + gridDim.x, ...
+// in the order of the one-tile-per-CTA grid (conv_unit), so the CTAs in flight work on neighbouring tiles as before (L2
+// reuse of the input rows and weights), and its consumer warpgroups take alternate units, each computing the whole
+// 128 x BN tile. The producer runs ahead across unit boundaries (one ring, counters never reset), and the
+// mainloops of the two consumers alternate on the tensor pipe, so one consumer's epilogue runs under the other one's MMAs.
+constexpr int kConvThreads = 384;
+constexpr int kStageStride = 36;                  // floats per staged pixel row: a 32-channel chunk + 4 (conflict-free rows)
+constexpr int kEpiFloats = kBM * kStageStride + 2 * 128 + 8 * 128;     // per consumer: staging, scale, bias, ToRGB weights
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;                  // 128 x 40 + 256 x 232 <= 64 K registers
 
-template <int kBN>
-__host__ __device__ constexpr int conv_stage_stride() { return (kBN > 32 ? kBN : 32) + 4; }   // floats per parked row
+struct ConvUnit {
+    ConvPhase P;
+    int tx, ty, tile_n, b, ksplit, k_begin, total_k;
+};
+
+// work unit u of the launch: u = ((b * splits + ksplit) * tiles_n + tile_n) * tiles_m + (spatial tile of the phases)
+__device__ __forceinline__ ConvUnit conv_unit(const ConvKernelArgs& a, int u) {
+    ConvUnit U;
+    const int t = u % a.tiles_m, r = u / a.tiles_m;
+    U.tile_n = r % a.tiles_n;
+    const int z = r / a.tiles_n;
+    U.b = z / a.splits;
+    U.ksplit = z - U.b * a.splits;
+    U.P = conv_phase_of(a, t);
+    const int tile_m = t - U.P.t0;
+    U.ty = tile_m / U.P.tiles_x;
+    U.tx = tile_m - U.ty * U.P.tiles_x;
+    const int all_k = U.P.ng * a.kc_steps;
+    U.k_begin = (int)((long long)all_k * U.ksplit / a.splits);
+    U.total_k = (int)((long long)all_k * (U.ksplit + 1) / a.splits) - U.k_begin;
+    return U;
+}
 
 template <int kAct, bool kClamp, int kBN>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                    const __grid_constant__ CUtensorMap tmB,
                                                                    const ConvKernelArgs a, int n_stages) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [stages][A 16 KB][B BN*128 B] | barriers | per-channel scale, bias | fused ToRGB weights [8][128]
+    // carve: [stages][A 16 KB][B BN*128 B] | barriers | per consumer warpgroup: [128 px][kStageStride] fp32 staging,
+    // per-channel scale, bias | fused ToRGB weights [8][128]
     // round up inside the shared window (pointer arithmetic on smem_raw keeps the address space known to the compiler)
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t a_bytes = (uint32_t)kBM * 128, b_bytes = (uint32_t)kBN * 128;
     const uint32_t stage_bytes = a_bytes + b_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + n_stages * stage_bytes);
     uint64_t* empty_bar = full_bar + kMaxStages;
-    float* s_scale = reinterpret_cast<float*>(empty_bar + kMaxStages);
-    float* s_bias = s_scale + 128;
-    float* s_rgbw = s_bias + 128;
-    float* s_acc = reinterpret_cast<float*>(smem);            // parked accumulators (after the k-loop)
-    constexpr int kSS = conv_stage_stride<kBN>();
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tile_n = blockIdx.y;
-    const ConvPhase P = conv_phase_of(a, (int)blockIdx.x);      // t0 counts spatial tiles here (blockIdx.x)
-    const int tile_m = (int)blockIdx.x - P.t0;
-    const int b = blockIdx.z / a.splits, ksplit = blockIdx.z - b * a.splits;
-    const int ty = tile_m / P.tiles_x, tx = tile_m % P.tiles_x;
-    const int n0 = tile_n * kBN;
-    const int all_k = P.ng * a.kc_steps;
-    const int k_begin = (int)((long long)all_k * ksplit / a.splits), k_end = (int)((long long)all_k * (ksplit + 1) / a.splits);
-    const int total_k = k_end - k_begin;
-
-    if (warp == 8 && lane == 0) {
+    const int wg = warp >> 2;
+    if (threadIdx.x == 0) {
         tc::tma_prefetch_desc(&tmA);
         tc::tma_prefetch_desc(&tmB);
-        for (int s = 0; s < n_stages; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 8); }
+        for (int s = 0; s < n_stages; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 4); }
         tc::fence_barrier_init();
-    }
-    if (warp < 8) {
-        // per-channel epilogue constants: accumulator scale (1/weight scale x demodulation x gain) and bias x gain; channels
-        // beyond Cout get zeros so the hot loop needs no channel predicate
-        const int i = threadIdx.x;
-        if (i < 128) {
-            const int ch = n0 + i;
-            float sc = 0.f, bi = 0.f;
-            if (i < kBN && ch < a.Cout) {
-                sc = a.acc_scale * a.pre_gain;
-                if (a.dscale) sc *= __ldg(a.dscale + (size_t)b * a.Cout + ch);
-                if (a.bias) bi = __ldg(a.bias + ch) * a.pre_gain;
-            }
-            s_scale[i] = sc;
-            s_bias[i] = bi;
-        }
-        if (a.rgb_w) {
-            // modulated ToRGB weights of this tile's sample as fp32 [8][128] (rows beyond rgb_cout are zero)
-            for (int j = i; j < 8 * 128; j += 256) {
-                const int c = j >> 7, k = j & 127;
-                s_rgbw[j] = (c < a.rgb_cout && k < a.Cout) ? __half2float(__ldg(a.rgb_w + ((size_t)b * a.rgb_w_rows + c) * a.Cout + k)) : 0.f;
-            }
-        }
     }
     __syncthreads();
 
-    if (warp == 8) {
-        // ===== TMA producer =====
-        if (lane == 0) {
+    if (wg == 0) {
+        // ===== TMA producer: every k-step of every unit of this CTA, in order, through one ring =====
+        tc::setmaxnreg_dec<kProducerRegs>();
+        if (threadIdx.x == 0) {
             int stage = 0; uint32_t phase = 0;
-            int g = k_begin / a.kc_steps, kc = k_begin - g * a.kc_steps;
-            g += P.g0;
-            for (int k = 0; k < total_k; ++k) {
-                const int x0 = tx * a.BW * a.stride + a.dx[g], y0 = ty * a.BH * a.stride + a.dy[g];
-                const int kb = a.tap[g] * a.Cin;
-                tc::mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* sa = smem + stage * stage_bytes;
-                uint8_t* sb = sa + a_bytes;
-                tc::mbar_expect_tx(&full_bar[stage], stage_bytes);
-                tc::tma_load_5d(sa, &tmA, &full_bar[stage], kc * kBK, x0, y0, b, a.a_plane[g]);
-                tc::tma_load_4d(sb, &tmB, &full_bar[stage], kb + kc * kBK, n0, a.w_per_sample ? b : 0, a.b_plane[g]);
-                if (++stage == n_stages) { stage = 0; phase ^= 1; }
-                if (++kc == a.kc_steps) { kc = 0; ++g; }
+            for (int u = blockIdx.x; u < a.n_units; u += gridDim.x) {
+                const ConvUnit U = conv_unit(a, u);
+                int g = U.k_begin / a.kc_steps, kc = U.k_begin - g * a.kc_steps;
+                g += U.P.g0;
+                const int n0 = U.tile_n * kBN;
+                for (int k = 0; k < U.total_k; ++k) {
+                    const int x0 = U.tx * a.BW * a.stride + a.dx[g], y0 = U.ty * a.BH * a.stride + a.dy[g];
+                    const int kb = a.tap[g] * a.Cin;
+                    tc::mbar_wait(&empty_bar[stage], phase ^ 1);
+                    uint8_t* sa = smem + stage * stage_bytes;
+                    uint8_t* sb = sa + a_bytes;
+                    tc::mbar_expect_tx(&full_bar[stage], stage_bytes);
+                    tc::tma_load_5d(sa, &tmA, &full_bar[stage], kc * kBK, x0, y0, U.b, a.a_plane[g]);
+                    tc::tma_load_4d(sb, &tmB, &full_bar[stage], kb + kc * kBK, n0, a.w_per_sample ? U.b : 0, a.b_plane[g]);
+                    if (++stage == n_stages) { stage = 0; phase ^= 1; }
+                    if (++kc == a.kc_steps) { kc = 0; ++g; }
+                }
             }
         }
         return;
     }
+    tc::setmaxnreg_inc<kConsumerRegs>();
 
-    // ===== consumers: warpgroup wg computes tile rows [64 wg, 64 wg + 64) x BN channels =====
-    const int wg = warp >> 2, wq = warp & 3;
-    float acc[kBN / 2];
-#pragma unroll
-    for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
-    {
-        int stage = 0; uint32_t phase = 0, prev = 0;
-        for (int k = 0; k < total_k; ++k) {
-            tc::mbar_wait(&full_bar[stage], phase);
-            const uint32_t sa = tc::smem_u32(smem + stage * stage_bytes);
-            const uint64_t da = tc::wgmma_desc_k128(sa + (uint32_t)wg * 64 * 128), db = tc::wgmma_desc_k128(sa + a_bytes);
-            tc::wgmma_fence();
-#pragma unroll
-            for (int j = 0; j < kBK / 16; ++j) tc::wgmma_ss(acc, da + (uint64_t)(j * 2), db + (uint64_t)(j * 2));
-            tc::wgmma_commit();
-            tc::wgmma_wait<1>();                              // the MMAs of the previous k-step have retired
-            if (k > 0 && lane == 0) tc::mbar_arrive(&empty_bar[prev]);
-            prev = stage;
-            if (++stage == n_stages) { stage = 0; phase ^= 1; }
-        }
-        tc::wgmma_wait<0>();
-        tc::wgmma_hold(acc);
-    }
-    // every consumer is past its last MMA and every TMA load has landed: the stage ring is free for the parked tile
-    tc::named_bar_sync(1, 256);
-    {
-        const int r0 = wg * 64 + wq * 16 + (lane >> 2), c = 2 * (lane & 3);
-#pragma unroll
-        for (int i = 0; i < kBN / 8; ++i)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-                *reinterpret_cast<float2*>(s_acc + (r0 + 8 * h) * kSS + 8 * i + c) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-    }
-    tc::named_bar_sync(1, 256);
+    // ===== consumers: warpgroup cw takes units i = cw, cw + 2, ... of this CTA's list =====
+    const int cw = wg - 1, wq = warp & 3;
+    const int m = threadIdx.x & 127;              // epilogue: thread = pixel (tile row m)
+    float* stg = reinterpret_cast<float*>(empty_bar + kMaxStages) + cw * kEpiFloats;
+    float* s_scale = stg + kBM * kStageStride;
+    float* s_bias = s_scale + 128;
+    float* s_rgbw = s_bias + 128;
+    // named barriers: 1 + cw = this consumer's turn for the mainloop (a consumer starts unit i once the other one has waited
+    // on every stage of unit i - 1; besides the alternation, this keeps each full-barrier wait within one phase of the
+    // barrier's state, the ring being shared); 3 + cw = this warpgroup's 128 threads (epilogue)
+    int it = 0;                                   // ring position: k-steps of the units before unit i
+    for (int i = 0;; ++i) {
+        const int u = blockIdx.x + i * gridDim.x;
+        if (u >= a.n_units) break;
+        const ConvUnit U = conv_unit(a, u);
+        if ((i & 1) != cw) { it += U.total_k; continue; }
 
-    // ===== epilogue: thread = pixel (tile row m); two threads per pixel split the 32-channel chunks, except for the fused
-    // ToRGB, whose dot products need every channel of the pixel in one thread =====
-    const int m = threadIdx.x & 127, part = threadIdx.x >> 7;
-    if (a.rgb_w && part == 1) return;
-    const int gy = ty * a.BH + m / a.BW, gx = tx * a.BW + m % a.BW;
-    const bool pix_ok = (gy < P.gH) && (gx < P.gW);
-    if (!pix_ok) return;
-    const int Y = gy * a.sy + P.oy, X = gx * a.sx + P.ox;
-    const size_t pix = ((size_t)b * a.oH + Y) * a.oW + X;
-    const float nz = a.noise ? __ldg(a.noise + (size_t)b * a.noise_bstride + (size_t)Y * a.oW + X) * a.pre_gain : 0.f;
-    const int out_mode = a.out_mode;
-    // vector path for a 32-channel chunk: the chunk is full (checked per chunk below: the channel tile may extend past Cout)
-    // and its stores are 32-byte aligned (chunk offsets are multiples of 32 channels, so the tile's alignment decides)
-    const bool vec_aligned = a.base_aligned && (out_mode <= 1 ? ((a.y_cstride % 16) == 0 && ((a.y_coff + n0) % 16) == 0)
-                                                              : ((a.y_cstride % 8) == 0 && ((a.y_coff + n0) % 8) == 0));
-    const float* row = s_acc + m * kSS;
-    float dot[8];
+        // tile rows 0-63 (acc0) and 64-127 (acc1): per k16 slice two m64nBNk16 MMAs on the same B operand
+        float acc0[kBN / 2], acc1[kBN / 2];
 #pragma unroll
-    for (int c = 0; c < 8; ++c) dot[c] = 0.f;
-    const int c_step = a.rgb_w ? 32 : 64;
-    for (int c0 = a.rgb_w ? 0 : 32 * part; c0 < kBN; c0 += c_step) {
-        uint32_t v[32];
+        for (int j = 0; j < kBN / 2; ++j) { acc0[j] = 0.f; acc1[j] = 0.f; }
+        if (i > 0) tc::named_bar_sync(1 + cw, 256);
+        {
+            int stage = it % n_stages; uint32_t phase = (uint32_t)(it / n_stages) & 1u;
+            int prev = 0;
+            for (int k = 0; k < U.total_k; ++k) {
+                tc::mbar_wait(&full_bar[stage], phase);
+                const uint32_t sa = tc::smem_u32(smem + stage * stage_bytes);
+                const uint64_t da0 = tc::wgmma_desc_k128(sa), da1 = tc::wgmma_desc_k128(sa + 64 * 128);
+                const uint64_t db = tc::wgmma_desc_k128(sa + a_bytes);
+                tc::wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-            const float4 t = *reinterpret_cast<const float4*>(row + c0 + i);
-            v[i] = __float_as_uint(t.x); v[i + 1] = __float_as_uint(t.y); v[i + 2] = __float_as_uint(t.z); v[i + 3] = __float_as_uint(t.w);
-        }
-        const int ch0 = n0 + c0;
-        if (a.partial) {
-            // split-K: raw accumulators of this k-range; conv_splitk_finish_kernel sums the ranges and applies the epilogue
-            float* pp = a.partial + P.p0 + ((((size_t)ksplit * (gridDim.z / a.splits) + b) * P.gH + gy) * P.gW + gx) * a.Cout_pad + ch0;
-            const int ncols = min(32, kBN - c0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-                if (8 * j < ncols && ch0 + 8 * j < a.Cout_pad) {
-                    const uint32_t o[8] = {v[8 * j], v[8 * j + 1], v[8 * j + 2], v[8 * j + 3], v[8 * j + 4], v[8 * j + 5], v[8 * j + 6], v[8 * j + 7]};
-                    st_global_256(pp + 8 * j, o);
+                for (int j = 0; j < kBK / 16; ++j) {
+                    tc::wgmma_ss(acc0, da0 + (uint64_t)(j * 2), db + (uint64_t)(j * 2));
+                    tc::wgmma_ss(acc1, da1 + (uint64_t)(j * 2), db + (uint64_t)(j * 2));
                 }
-            continue;
+                tc::wgmma_commit();
+                tc::wgmma_wait<1>();                          // the MMAs of the previous k-step have retired
+                if (k > 0 && lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+                prev = stage;
+                if (++stage == n_stages) { stage = 0; phase ^= 1; }
+            }
+            if (u + (int)gridDim.x < a.n_units) tc::named_bar_arrive(2 - cw, 256);
+            tc::wgmma_wait<0>();
+            if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
+            tc::wgmma_hold(acc0);
+            tc::wgmma_hold(acc1);
         }
-        if (ch0 >= a.Cout) continue;
-        const size_t off = pix * a.y_cstride + a.y_coff + ch0;
-        const bool vec_ok = vec_aligned && ch0 + 32 <= a.Cout;
-        if (a.rgb_w) {
-            // fused ToRGB of the next layer: dot products of this pixel's fp16-rounded outputs with the 1x1 weights
-            float xq[32];
-            conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, off, nz, vec_ok, b, Y, X, xq, a.rgb_skip_x == 0);
+        it += U.total_k;
+
+        const ConvPhase& P = U.P;
+        const int b = U.b, n0 = U.tile_n * kBN;
+        // s_scale / s_bias / s_rgbw hold the constants of this warpgroup's previous unit, i - 2
+        bool reload = i < 2;
+        if (!reload) {
+            const ConvUnit V = conv_unit(a, u - 2 * (int)gridDim.x);
+            reload = V.b != b || V.tile_n != U.tile_n;
+        }
+        if (reload) {
+            // per-channel epilogue constants: accumulator scale (1/weight scale x demodulation x gain) and bias x gain;
+            // channels beyond Cout get zeros so the hot loop needs no channel predicate
+            tc::named_bar_sync(3 + cw, 128);                 // the previous tile's epilogue is done with them
+            const int ch = n0 + m;
+            float sc = 0.f, bi = 0.f;
+            if (m < kBN && ch < a.Cout) {
+                sc = a.acc_scale * a.pre_gain;
+                if (a.dscale) sc *= __ldg(a.dscale + (size_t)b * a.Cout + ch);
+                if (a.bias) bi = __ldg(a.bias + ch) * a.pre_gain;
+            }
+            s_scale[m] = sc;
+            s_bias[m] = bi;
+            if (a.rgb_w) {
+                // modulated ToRGB weights of this tile's sample as fp32 [8][128] (rows beyond rgb_cout are zero)
+                for (int j = m; j < 8 * 128; j += 128) {
+                    const int c = j >> 7, kk = j & 127;
+                    s_rgbw[j] = (c < a.rgb_cout && kk < a.Cout) ? __half2float(__ldg(a.rgb_w + ((size_t)b * a.rgb_w_rows + c) * a.Cout + kk)) : 0.f;
+                }
+            }
+        }
+
+        // ===== epilogue, one 32-channel chunk at a time: the warpgroup stages the chunk's accumulators as fp32
+        // [128 pixels][32] so that a thread owns one pixel and reads its 32 consecutive channels, the form conv_store_chunk takes
+        const int gy = U.ty * a.BH + m / a.BW, gx = U.tx * a.BW + m % a.BW;
+        const bool pix_ok = (gy < P.gH) && (gx < P.gW);
+        const int Y = gy * a.sy + P.oy, X = gx * a.sx + P.ox;
+        const size_t pix = ((size_t)b * a.oH + Y) * a.oW + X;
+        // split-K: raw accumulators of this k-range go to the partials; conv_splitk_finish_kernel sums the ranges and applies
+        // the epilogue
+        const size_t part_off = P.p0 + ((((size_t)U.ksplit * a.B + b) * P.gH + gy) * P.gW + gx) * a.Cout_pad;
+        const float nz = (a.noise && pix_ok) ? __ldg(a.noise + (size_t)b * a.noise_bstride + (size_t)Y * a.oW + X) * a.pre_gain : 0.f;
+        const int out_mode = a.out_mode;
+        // vector path for a 32-channel chunk: the chunk is full (checked per chunk below: the channel tile may extend past
+        // Cout) and its stores are 32-byte aligned (chunk offsets are multiples of 32 channels, so the tile's alignment decides)
+        const bool vec_aligned = a.base_aligned && (out_mode <= 1 ? ((a.y_cstride % 16) == 0 && ((a.y_coff + n0) % 16) == 0)
+                                                                  : ((a.y_cstride % 8) == 0 && ((a.y_coff + n0) % 8) == 0));
+        float* row = stg + m * kStageStride;
+        float dot[8];
+#pragma unroll
+        for (int c = 0; c < 8; ++c) dot[c] = 0.f;
+#pragma unroll
+        for (int q = 0; q < kBN / 32; ++q) {
+            const int c0 = 32 * q;
+            tc::named_bar_sync(3 + cw, 128);                 // the previous chunk has been read; the constants are visible
+            {
+                const int r0 = wq * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+                for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int i4 = 4 * (4 * q + ii) + 2 * h;
+                        *reinterpret_cast<float2*>(stg + (r0 + 8 * h) * kStageStride + 8 * ii + c) = make_float2(acc0[i4], acc0[i4 + 1]);
+                        *reinterpret_cast<float2*>(stg + (r0 + 64 + 8 * h) * kStageStride + 8 * ii + c) = make_float2(acc1[i4], acc1[i4 + 1]);
+                    }
+            }
+            tc::named_bar_sync(3 + cw, 128);
+            if (!pix_ok) continue;
+            uint32_t v[32];
+#pragma unroll
+            for (int i4 = 0; i4 < 32; i4 += 4) {
+                const float4 t = *reinterpret_cast<const float4*>(row + i4);
+                v[i4] = __float_as_uint(t.x); v[i4 + 1] = __float_as_uint(t.y); v[i4 + 2] = __float_as_uint(t.z); v[i4 + 3] = __float_as_uint(t.w);
+            }
+            const int ch0 = n0 + c0;
+            if (a.partial) {
+                float* pp = a.partial + part_off + ch0;
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    if (ch0 + 8 * j < a.Cout_pad) {
+                        const uint32_t o[8] = {v[8 * j], v[8 * j + 1], v[8 * j + 2], v[8 * j + 3], v[8 * j + 4], v[8 * j + 5], v[8 * j + 6], v[8 * j + 7]};
+                        st_global_256(pp + 8 * j, o);
+                    }
+                continue;
+            }
+            if (ch0 >= a.Cout) continue;
+            const size_t off = pix * a.y_cstride + a.y_coff + ch0;
+            const bool vec_ok = vec_aligned && ch0 + 32 <= a.Cout;
+            if (a.rgb_w) {
+                // fused ToRGB of the next layer: dot products of this pixel's fp16-rounded outputs with the 1x1 weights. The
+                // rounded outputs go back to the pixel's own staging row (already read into v), not to registers.
+                float* xq = row;
+                conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, off, nz, vec_ok, b, Y, X, xq, a.rgb_skip_x == 0);
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    if (c < a.rgb_cout) {
+                        const float4* wr = reinterpret_cast<const float4*>(s_rgbw + c * 128 + c0);
+                        float acc_c = dot[c];
+#pragma unroll
+                        for (int qd = 0; qd < 8; ++qd) {
+                            const float4 w4 = wr[qd];
+                            acc_c = fmaf(xq[4 * qd], w4.x, acc_c); acc_c = fmaf(xq[4 * qd + 1], w4.y, acc_c);
+                            acc_c = fmaf(xq[4 * qd + 2], w4.z, acc_c); acc_c = fmaf(xq[4 * qd + 3], w4.w, acc_c);
+                        }
+                        dot[c] = acc_c;
+                    }
+                }
+            } else {
+                conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, off, nz, vec_ok, b, Y, X);
+            }
+        }
+        if (a.rgb_w && pix_ok) {
+            // out = upsample2d(prev)[b, Y, X, :] + round16(clamp(dot * scale + bias)), written NCHW (lanes = consecutive X)
+            const int ph = a.oH >> 1, pw = a.oW >> 1, C = a.rgb_cout;
+            const int iy = Y >> 1, py = Y & 1, ix = X >> 1, px = X & 1;
+            float w4[2][2];
+            const float* pp[2][2];
+#pragma unroll
+            for (int aa = 0; aa < 2; ++aa)
+#pragma unroll
+                for (int cc = 0; cc < 2; ++cc) {
+                    const int ry = iy - 1 + py + aa, rx = ix - 1 + px + cc;
+                    const bool ok = ry >= 0 && ry < ph && rx >= 0 && rx < pw;
+                    w4[aa][cc] = ok ? __ldg(a.rgb_f + (3 - (py + 2 * aa)) * 4 + (3 - (px + 2 * cc))) * 4.f : 0.f;
+                    pp[aa][cc] = a.rgb_prev + (((size_t)b * ph + (ok ? ry : 0)) * pw + (ok ? rx : 0)) * C;
+                }
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
-                if (c < a.rgb_cout) {
-                    const float4* wr = reinterpret_cast<const float4*>(s_rgbw + c * 128 + c0);
-                    float acc_c = dot[c];
+                if (c < C) {
+                    float up = 0.f;
 #pragma unroll
-                    for (int qd = 0; qd < 8; ++qd) {
-                        const float4 w4 = wr[qd];
-                        acc_c = fmaf(xq[4 * qd], w4.x, acc_c); acc_c = fmaf(xq[4 * qd + 1], w4.y, acc_c);
-                        acc_c = fmaf(xq[4 * qd + 2], w4.z, acc_c); acc_c = fmaf(xq[4 * qd + 3], w4.w, acc_c);
-                    }
-                    dot[c] = acc_c;
+                    for (int aa = 0; aa < 2; ++aa)
+#pragma unroll
+                        for (int cc = 0; cc < 2; ++cc) up = fmaf(w4[aa][cc], __ldg(pp[aa][cc] + c), up);
+                    float x = fmaf(dot[c], a.rgb_acc_scale, a.rgb_bias ? __ldg(a.rgb_bias + c) : 0.f);
+                    if (a.rgb_clamp >= 0.f) x = fminf(fmaxf(x, -a.rgb_clamp), a.rgb_clamp);
+                    x = __half2float(__float2half_rn(x));
+                    a.rgb_out[(((size_t)b * C + c) * a.oH + Y) * a.oW + X] = up + x;
                 }
-            }
-        } else {
-            conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, off, nz, vec_ok, b, Y, X);
-        }
-    }
-    if (a.rgb_w) {
-        // out = upsample2d(prev)[b, Y, X, :] + round16(clamp(dot * scale + bias)), written NCHW (lanes = consecutive X)
-        const int ph = a.oH >> 1, pw = a.oW >> 1, C = a.rgb_cout;
-        const int iy = Y >> 1, py = Y & 1, ix = X >> 1, px = X & 1;
-        float w4[2][2];
-        const float* pp[2][2];
-#pragma unroll
-        for (int aa = 0; aa < 2; ++aa)
-#pragma unroll
-            for (int cc = 0; cc < 2; ++cc) {
-                const int ry = iy - 1 + py + aa, rx = ix - 1 + px + cc;
-                const bool ok = ry >= 0 && ry < ph && rx >= 0 && rx < pw;
-                w4[aa][cc] = ok ? __ldg(a.rgb_f + (3 - (py + 2 * aa)) * 4 + (3 - (px + 2 * cc))) * 4.f : 0.f;
-                pp[aa][cc] = a.rgb_prev + (((size_t)b * ph + (ok ? ry : 0)) * pw + (ok ? rx : 0)) * C;
-            }
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-            if (c < C) {
-                float u = 0.f;
-#pragma unroll
-                for (int aa = 0; aa < 2; ++aa)
-#pragma unroll
-                    for (int cc = 0; cc < 2; ++cc) u = fmaf(w4[aa][cc], __ldg(pp[aa][cc] + c), u);
-                float x = fmaf(dot[c], a.rgb_acc_scale, a.rgb_bias ? __ldg(a.rgb_bias + c) : 0.f);
-                if (a.rgb_clamp >= 0.f) x = fminf(fmaxf(x, -a.rgb_clamp), a.rgb_clamp);
-                x = __half2float(__float2half_rn(x));
-                a.rgb_out[(((size_t)b * C + c) * a.oH + Y) * a.oW + X] = u + x;
             }
         }
     }
@@ -625,7 +684,7 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     ConvKernelArgs a;
     memset(&a, 0, sizeof(a));
     static const int pa[3] = {0, 0, 1}, pb[3] = {0, 1, 0};     // hi*hi, hi*lo, lo*hi
-    int g = 0, tiles_m_total = 0, max_total_k = 0, min_total_k = 1 << 30;
+    int g = 0, tiles_m_total = 0, min_total_k = 1 << 30;
     a.n_phases = n_phases;
     a.kc_steps = p->C / kBK;
     for (int q = 0; q < n_phases; ++q) {
@@ -641,10 +700,9 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
         P.ng = g - P.g0;
         P.gH = r->gH; P.gW = r->gW; P.oy = r->oy; P.ox = r->ox;
         P.tiles_x = ceil_div(r->gW, BW); P.tiles_y = ceil_div(r->gH, BH);
-        P.t0 = tiles_m_total;                                   // spatial tiles of the phase: blockIdx.x range
+        P.t0 = tiles_m_total;                                   // spatial tiles of the phase: a range of the tile index
         tiles_m_total += P.tiles_x * P.tiles_y;
         const int tk = P.ng * a.kc_steps;
-        if (tk > max_total_k) max_total_k = tk;
         if (tk < min_total_k) min_total_k = tk;
     }
     a.Cin = p->C;
@@ -719,17 +777,23 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
             }
         }
     }
-    // 4 stages by default; grids with at most one CTA per SM and long k-loops (the 4^2..32^2 backbone layers) are bound by
-    // TMA latency x bytes in flight instead and get the deepest ring the shared memory holds
-    const bool deep = (long)grid.x * grid.y * grid.z <= sm_count() && max_total_k / a.splits > 6;
+    // persistent grid: at most one CTA per SM (the kernel's registers and shared memory allow no more) walking the work units
+    // (grid.x spatial tiles x grid.y channel tiles x grid.z samples and k-splits) in the order of the one-tile-per-CTA grid
+    a.B = p->B; a.tiles_m = (int)grid.x; a.tiles_n = (int)grid.y;
+    const long units = (long)grid.x * grid.y * grid.z;
+    a.n_units = (int)units;
+    const int n_ctas = (int)(units < sm_count() ? units : sm_count());
+    // the deepest ring that fits next to the two epilogue buffers: 5 stages at BN = 128, 6 below (one CTA per SM either way)
     const size_t stage_bytes = (size_t)kBM * 128 + (size_t)BN * 128;
-    const int n_stages = deep ? kMaxStages : 4;
-    const size_t smem = n_stages * stage_bytes + 2 * kMaxStages * 8 + (2 * 128 + 8 * 128) * sizeof(float) + 1024;
+    const size_t smem_fixed = 2 * kMaxStages * 8 + 2 * (size_t)kEpiFloats * sizeof(float) + 1024;
+    int n_stages = kMaxStages;
+    while (n_stages * stage_bytes + smem_fixed > kSmemPerBlock) --n_stages;
+    const size_t smem = n_stages * stage_bytes + smem_fixed;
 #define P3D_LAUNCH_CONV_N(ACT, CL, BNV)                                                                                       \
     do {                                                                                                                      \
         P3D_CUDA_TRY(cudaFuncSetAttribute(conv_gemm_kernel<ACT, CL, BNV>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
                                           (int)smem));                                                                        \
-        conv_gemm_kernel<ACT, CL, BNV><<<grid, kConvThreads, smem, (cudaStream_t)stream>>>(tmA, tmB, a, n_stages);           \
+        conv_gemm_kernel<ACT, CL, BNV><<<n_ctas, kConvThreads, smem, (cudaStream_t)stream>>>(tmA, tmB, a, n_stages);         \
     } while (0)
 #define P3D_LAUNCH_CONV(ACT, CL)                                                                                              \
     do {                                                                                                                      \
