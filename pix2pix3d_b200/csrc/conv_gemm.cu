@@ -60,7 +60,7 @@ struct ConvKernelArgs {
     const float* bias; const float* noise; const float* dscale;
     int64_t noise_bstride;            // elements between the noise images of consecutive samples (0: one image for the batch)
     float alpha, clamp, acc_scale;
-    int base_aligned;                 // y / y_lo are 32-byte aligned (256-bit stores allowed)
+    int base_aligned;                 // y / y_lo are 32-byte aligned and residual rows 16-byte aligned (vector epilogue allowed)
     int splits;                       // split-K: work unit sample index b * splits + s; s covers k-steps [s*total/splits, (s+1)*total/splits)
     float* partial;                   // split-K: raw fp32 accumulators, per phase [splits][B][gH][gW][Cout_pad] (finished by a second kernel)
     int Cout_pad;
@@ -715,6 +715,8 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     a.noise_bstride = p->noise_batch_stride;
     a.alpha = p->alpha; a.clamp = p->clamp; a.acc_scale = p->acc_scale;
     a.base_aligned = ((((uintptr_t)p->y) | ((uintptr_t)p->y_lo)) & 31) == 0;
+    // the vector path also reads the residual with 16-byte loads; its pixel rows lie Cout floats apart
+    if (p->residual && p->Cout % 4 != 0) a.base_aligned = 0;
     a.up_prev = p->up_prev; a.up_f = p->up_filter; a.round16 = p->round16; a.out_nchw = p->out_nchw;
     a.stride = stride; a.residual = p->residual;
     if (p->rgb_w) {
