@@ -149,13 +149,23 @@ def ray_limits_box(rays_o, rays_d, box_side_length):
     return tn.reshape(*lead, 1), tf.reshape(*lead, 1)
 
 
+def _out_view(buf, shape, dtype, dev):
+    """The leading elements of a caller's flat output buffer, viewed as `shape`."""
+    n = int(np.prod(shape))
+    assert buf.dtype == dtype and buf.device == dev and buf.is_contiguous() and buf.numel() >= n, 'render_fwd out= buffer'
+    return buf.reshape(-1)[:n].view(shape)
+
+
 def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_warp, white_back=False, debug=False, impl=None,
-               stratified=None, plane_index=None):
+               stratified=None, plane_index=None, out=None):
     """Fused ImportanceRenderer.forward. Returns (feat [B,R,C], depth [B,R,1], wsum [B,R,1][, debug dict]).
     `stratified` (instead of `depths_coarse`): the ingredients of sample_stratified, combined inside the kernel --
     dict(jitter=[B,R,Sc] U[0,1) draw, table=[Sc], delta=float) for scalar ray limits or dict(jitter, table, ray_start=[B,R],
     ray_end=[B,R]) for per-ray limits (p3d_render_args_t::depth_mode 1 / 2).
-    `plane_index` ([B] int32): plane set of each image; lets B views share fewer plane sets (planes batch < B)."""
+    `plane_index` ([B] int32): plane set of each image; lets B views share fewer plane sets (planes batch < B).
+    `out` (optional dict): contiguous buffers to write instead of fresh ones, keyed like the outputs and the debug dict
+    (feat, depth, wsum, weights_final, perm, weights_coarse, depths_fine, inds); each may be longer than the launch needs,
+    and the launch writes only its leading elements."""
     Bp, _, H, W, C = planes_nhwc.shape
     B = ray_origins.shape[0]
     if plane_index is None and Bp != B:
@@ -184,9 +194,14 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
     Sf = 0 if u is None else int(u.shape[-1])
     uu = None if u is None else _f32c(u)
     dev = planes_nhwc.device
-    feat = torch.empty(B, R, dec.out_channels, device=dev, dtype=torch.float32)
-    depth = torch.empty(B, R, 1, device=dev, dtype=torch.float32)
-    wsum = torch.empty(B, R, 1, device=dev, dtype=torch.float32)
+    out = out or {}
+
+    def alloc(key, shape, dtype):
+        return _out_view(out[key], shape, dtype, dev) if key in out else torch.empty(*shape, device=dev, dtype=dtype)
+
+    feat = alloc('feat', (B, R, dec.out_channels), torch.float32)
+    depth = alloc('depth', (B, R, 1), torch.float32)
+    wsum = alloc('wsum', (B, R, 1), torch.float32)
     ws = torch.empty(4, device=dev, dtype=torch.int32)
     a = _lib.RenderArgs()
     a.planes_nhwc, a.ray_origins, a.ray_dirs = planes_nhwc.data_ptr(), o.data_ptr(), d.data_ptr()
@@ -218,13 +233,13 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
     want_debug = debug or render_debug_sink is not None
     if want_debug:
         S = Sc + Sf
-        dbg['weights_final'] = torch.empty(B, R, S - 1, device=dev, dtype=torch.float32)
-        dbg['perm'] = torch.empty(B, R, S, device=dev, dtype=torch.int32)
+        dbg['weights_final'] = alloc('weights_final', (B, R, S - 1), torch.float32)
+        dbg['perm'] = alloc('perm', (B, R, S), torch.int32)
         a.dbg_weights_final, a.dbg_perm = dbg['weights_final'].data_ptr(), dbg['perm'].data_ptr()
         if Sf > 0:
-            dbg['weights_coarse'] = torch.empty(B, R, Sc - 1, device=dev, dtype=torch.float32)
-            dbg['depths_fine'] = torch.empty(B, R, Sf, device=dev, dtype=torch.float32)
-            dbg['inds'] = torch.empty(B, R, Sf, device=dev, dtype=torch.int32)
+            dbg['weights_coarse'] = alloc('weights_coarse', (B, R, Sc - 1), torch.float32)
+            dbg['depths_fine'] = alloc('depths_fine', (B, R, Sf), torch.float32)
+            dbg['inds'] = alloc('inds', (B, R, Sf), torch.int32)
             a.dbg_weights_coarse = dbg['weights_coarse'].data_ptr()
             a.dbg_depths_fine, a.dbg_inds = dbg['depths_fine'].data_ptr(), dbg['inds'].data_ptr()
     a.workspace = ws.data_ptr()
