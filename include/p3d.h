@@ -127,6 +127,10 @@ typedef struct {
     /* Optional [B] plane-set index per image: rays of image b gather from plane set plane_index[b] (NULL: b). Lets V camera
      * views of one latent (applications/generate_video.py:57-69) share ONE resident plane set: planes batch 1, B = V. */
     const int32_t* plane_index;
+    /* Optional [B,R,Sc+Sf] output (ABI 6; NULL: not written): the merged depths in sorted order, torch.sort(cat(coarse,
+     * fine)) (renderer.py:157-167), i.e. the depths at dbg_perm. What p3d_render_bwd needs to recompute a ray. Every other
+     * output is the same whether it is set or not. */
+    float* out_depths_sorted;
 } p3d_render_args_t;
 
 /* math_utils.get_ray_limits_box (training/volumetric_rendering/math_utils.py:46-98): slab test of N rays against the cube of
@@ -209,6 +213,42 @@ int p3d_ray_march(const float* colors, const float* densities, const float* dept
 int p3d_ray_march_bwd(const float* colors, const float* densities, const float* depths, const float* grad_rgb,
                       const float* grad_depth, const float* grad_weights, const float* depth_range, int N, int S,
                       int Cc, int white_back, float* grad_colors, float* grad_densities, p3d_stream_t stream);
+
+/* First-order backward of ImportanceRenderer.forward as p3d_render_fwd computes it (pix2pix3d_b200/csrc/render_fused_bwd.cu).
+ * Gradient reaches the planes and the decoder parameters only through the final march over the merged samples (the coarse
+ * march feeds importance sampling, which runs under no_grad). Each ray is recomputed from its sorted depths: gather,
+ * decoder (fp32, library expf / log1pf), march backward as p3d_ray_march_bwd, decoder backward, scatter of the bilinear taps. */
+typedef struct {
+    const float* planes_nhwc;    /* [B,3,H,W,32] fp32, dense */
+    const float* ray_origins;    /* [B,R,3] */
+    const float* ray_dirs;       /* [B,R,3] */
+    const float* depths_sorted;  /* [B,R,Sc+Sf]  p3d_render_args_t::out_depths_sorted of the forward */
+    /* EFFECTIVE decoder parameters per net (weight * weight_gain, bias * bias_gain), as p3d_decoder_mlp_fwd takes them */
+    const float* w1[2];          /* [64,32] */
+    const float* b1[2];          /* [64] */
+    const float* w2[2];          /* [33,64] */
+    const float* b2[2];          /* [33] */
+    int32_t n_nets, sigma_net;
+    uint32_t sigmoid_mask[2];
+    int32_t B, R, H, W, Sc, Sf;
+    float   coord_scale;         /* 2/box_warp */
+    int32_t white_back;
+    /* upstream gradients */
+    const float* g_feat;         /* [B,R,32*n_nets] */
+    const float* g_depth;        /* [B,R] or NULL */
+    const float* g_wsum;         /* [B,R] or NULL */
+    const float* depth_range;    /* device [2] = {min, max} of all depths; required with g_depth */
+    /* outputs (either may be NULL: that part of the work is skipped) */
+    float* g_planes_nhwc;        /* [B,3,H,W,32]: zeroed here, then the taps are scattered with vector atomics */
+    float* g_params;             /* [n_nets,4257] per net dL/dw1 | dL/db1 | dL/dw2 | dL/db2 (layout of p3d_decoder_mlp_bwd);
+                                    per-CTA partials are added in a fixed order: bit-identical from run to run */
+    float* workspace;            /* fp32 scratch of at least p3d_render_bwd_workspace_floats(n_nets) elements */
+    int64_t workspace_floats;
+} p3d_render_bwd_args_t;
+
+/* Sc, Sf <= 64 (else P3D_UNSUPPORTED). */
+int p3d_render_bwd_workspace_floats(int n_nets);
+int p3d_render_bwd(const p3d_render_bwd_args_t* args, p3d_stream_t stream);
 
 /* sample_importance + sample_pdf -- renderer.py:194-253. z_vals [N,S], weights [N,S-1], u [N,Sf];
  * out_samples [N,Sf], out_inds [N,Sf] (may be NULL). */

@@ -10,7 +10,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libp3d.so')
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 _lib = None
 
@@ -44,6 +44,19 @@ class RenderArgs(ctypes.Structure):  # p3d_render_args_t
         ('tc_variant', c_int32), ('depth_mode', c_int32),
         ('jitter', c_void_p), ('depth_table', c_void_p), ('ray_start', c_void_p), ('ray_end', c_void_p),
         ('depth_delta', c_float), ('reserved1', c_int32), ('plane_index', c_void_p),
+        ('out_depths_sorted', c_void_p),
+    ]
+
+
+class RenderBwdArgs(ctypes.Structure):  # p3d_render_bwd_args_t
+    _fields_ = [
+        ('planes_nhwc', c_void_p), ('ray_origins', c_void_p), ('ray_dirs', c_void_p), ('depths_sorted', c_void_p),
+        ('w1', c_void_p * 2), ('b1', c_void_p * 2), ('w2', c_void_p * 2), ('b2', c_void_p * 2),
+        ('n_nets', c_int32), ('sigma_net', c_int32), ('sigmoid_mask', c_uint32 * 2),
+        ('B', c_int32), ('R', c_int32), ('H', c_int32), ('W', c_int32), ('Sc', c_int32), ('Sf', c_int32),
+        ('coord_scale', c_float), ('white_back', c_int32),
+        ('g_feat', c_void_p), ('g_depth', c_void_p), ('g_wsum', c_void_p), ('depth_range', c_void_p),
+        ('g_planes_nhwc', c_void_p), ('g_params', c_void_p), ('workspace', c_void_p), ('workspace_floats', c_int64),
     ]
 
 
@@ -86,6 +99,8 @@ _SIGNATURES = {
     'p3d_sample_from_planes': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     'p3d_ray_march': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                               c_void_p, c_void_p]),
+    'p3d_render_bwd_workspace_floats': (c_int, [c_int]),
+    'p3d_render_bwd': (c_int, [ctypes.POINTER(RenderBwdArgs), c_void_p]),
     'p3d_sample_importance': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'p3d_bias_act': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                              c_float, c_float, c_int64, c_int, c_int64, c_void_p]),

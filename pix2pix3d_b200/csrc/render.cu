@@ -408,6 +408,7 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
             rbC[L.o_sd + cnt] = dC;
             rbC[L.o_ss + cnt] = rbC[L.o_sC + sC];
             if (a.dbg_perm) a.dbg_perm[(size_t)gC * S + cnt] = sC;
+            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gC * S + cnt] = dC;
         }
         if (vF) {
             const float* dc = rbF + L.o_dC;
@@ -420,6 +421,7 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
             rbF[L.o_sd + cnt] = dFv;
             rbF[L.o_ss + cnt] = rbF[L.o_sF + sF];
             if (a.dbg_perm) a.dbg_perm[(size_t)gF * S + cnt] = Sc + sF;
+            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gF * S + cnt] = dFv;
         }
         __syncthreads();
 
@@ -736,7 +738,7 @@ using namespace p3d;
 
 extern "C" {
 
-int p3d_abi_version(void) { return 5; }
+int p3d_abi_version(void) { return 6; }
 const char* p3d_build_info(void) { return "libp3d sm_90a " __DATE__ " " __TIME__; }
 const char* p3d_status_string(int status) {
     if (status == P3D_OK) return "ok";

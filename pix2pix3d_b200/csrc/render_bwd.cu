@@ -57,8 +57,6 @@ __global__ void __launch_bounds__(128) ray_march_bwd_kernel(const float* __restr
     float* wv = dot + Sp;        // w_i
     float* gsm = wv + Sp;        // dL / d dens_mid_i
     const int nI = S - 1;
-    const int K = (nI + 31) / 32;
-    const int i0 = lane * K;
     const float dlo = depth_range ? __ldg(depth_range) : 0.f, dhi = depth_range ? __ldg(depth_range + 1) : 0.f;
     for (int ray = blockIdx.x * nwarps + warp; ray < N; ray += gridDim.x * nwarps) {
         for (int i = lane; i < S; i += 32) {
@@ -87,95 +85,9 @@ __global__ void __launch_bounds__(128) ray_march_bwd_kernel(const float* __restr
             if (lane == 0) dot[j] = part;
         }
         __syncwarp();
-        // ---- forward recompute (same structure as warp_march) ----
-        float alpha[kMaxIvPerLane], tl[kMaxIvPerLane], ee[kMaxIvPerLane], aa[kMaxIvPerLane], dl[kMaxIvPerLane], xx[kMaxIvPerLane];
-        float prod = 1.f;
-#pragma unroll
-        for (int k = 0; k < kMaxIvPerLane; ++k) {
-            if (k < K) {
-                const int i = i0 + k;
-                float a = 0.f, e = 1.f, delta = 0.f, x = 0.f;
-                if (i < nI) {
-                    delta = __fsub_rn(d[i + 1], d[i]);
-                    x = __fsub_rn(__fmul_rn(__fadd_rn(s[i], s[i + 1]), 0.5f), 1.f);
-                    const float sp = x > 20.f ? x : log1pf(expf(x));
-                    e = expf(-__fmul_rn(sp, delta));
-                    a = 1.f - e;
-                }
-                alpha[k] = a; ee[k] = e; dl[k] = delta; xx[k] = x;
-                tl[k] = prod;
-                const float t = (i < nI) ? __fadd_rn(__fsub_rn(1.f, a), 1e-10f) : 1.f;
-                aa[k] = t;
-                prod = __fmul_rn(prod, t);
-            }
-        }
-        float incl = prod;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const float v = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl = __fmul_rn(incl, v);
-        }
-        float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-        if (lane == 0) excl = 1.f;
-        float sw = 0.f, swd = 0.f;
-#pragma unroll
-        for (int k = 0; k < kMaxIvPerLane; ++k) {
-            if (k < K) {
-                const int i = i0 + k;
-                if (i < nI) {
-                    tl[k] = __fmul_rn(excl, tl[k]);          // T_i
-                    const float wi = __fmul_rn(alpha[k], tl[k]);
-                    wv[i] = wi;
-                    sw += wi;
-                    swd = fmaf(wi, __fmul_rn(__fadd_rn(d[i], d[i + 1]), 0.5f), swd);
-                }
-            }
-        }
-        sw = warp_sum(sw);
-        swd = warp_sum(swd);
-        // ---- gradient w.r.t. the weights ----
         const float gd = g_depth ? __ldg(g_depth + ray) : 0.f;
-        const float draw = swd / sw;
-        const bool depth_ok = gd != 0.f && isfinite(draw) && draw >= dlo && draw <= dhi;
-        const float gd_w = depth_ok ? gd / sw : 0.f;
-        float gw[kMaxIvPerLane];
-        float local = 0.f;
-#pragma unroll
-        for (int k = 0; k < kMaxIvPerLane; ++k) {
-            gw[k] = 0.f;
-            if (k < K) {
-                const int i = i0 + k;
-                if (i < nI) {
-                    float g = 0.5f * (dot[i] + dot[i + 1]);
-                    if (white_back) g -= sumG;
-                    if (g_w) g += __ldg(g_w + (size_t)ray * nI + i);
-                    if (depth_ok) g = fmaf(gd_w, __fmul_rn(__fadd_rn(d[i], d[i + 1]), 0.5f) - draw, g);
-                    gw[k] = g;
-                    local = fmaf(g, wv[i], local);
-                }
-            }
-        }
-        // exclusive suffix sum of gw_k w_k over the lanes to the right
-        float sfx = local;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const float v = __shfl_down_sync(0xffffffffu, sfx, o);
-            if (lane + o < 32) sfx += v;
-        }
-        float run = __shfl_down_sync(0xffffffffu, sfx, 1);
-        if (lane == 31) run = 0.f;
-#pragma unroll
-        for (int k = kMaxIvPerLane - 1; k >= 0; --k) {
-            if (k < K) {
-                const int i = i0 + k;
-                if (i < nI) {
-                    const float g_alpha = gw[k] * tl[k] - run / aa[k];
-                    const float sg = xx[k] > 20.f ? 1.f : 1.f / (1.f + expf(-xx[k]));
-                    gsm[i] = g_alpha * ee[k] * dl[k] * sg;
-                    run = fmaf(gw[k], wv[i], run);
-                }
-            }
-        }
+        warp_march_bwd(d, s, dot, S, sumG, white_back, gd, dlo, dhi,
+                       [&](int i, float g) { return g_w ? g + __ldg(g_w + (size_t)ray * nI + i) : g; }, wv, gsm, lane);
         __syncwarp();
         // ---- outputs ----
         for (int j = lane; j < S; j += 32) {

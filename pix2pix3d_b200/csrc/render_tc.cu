@@ -257,6 +257,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
             rbC[L.o_sd + cnt] = dC;
             rbC[L.o_ss + cnt] = rbC[L.o_sC + sC];
             if (a.dbg_perm) a.dbg_perm[(size_t)gC * S + cnt] = sC;
+            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gC * S + cnt] = dC;
         }
         if (vF && grpF) {
             const float* dc = rbF + L.o_dC;
@@ -282,6 +283,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
             rbF[L.o_sd + cnt] = dFv;
             rbF[L.o_ss + cnt] = rbF[L.o_sF + sF];
             if (a.dbg_perm) a.dbg_perm[(size_t)gF * S + cnt] = Sc + sF;
+            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gF * S + cnt] = dFv;
         }
         __syncthreads();
 

@@ -198,6 +198,7 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
             rb[L.o_sd + cnt] = dC;
             rb[L.o_ss + cnt] = rb[L.o_sC + sidx];
             if (a.dbg_perm) a.dbg_perm[(size_t)gray * S + cnt] = sidx;
+            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gray * S + cnt] = dC;
         }
         if (vF) {
             const float* dc = rb + L.o_dC;
@@ -216,6 +217,7 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
             rb[L.o_sd + cnt] = dFv;
             rb[L.o_ss + cnt] = rb[L.o_sF + sidx];
             if (a.dbg_perm) a.dbg_perm[(size_t)gray * S + cnt] = Sc + sidx;
+            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gray * S + cnt] = dFv;
         }
         group_sync();
 

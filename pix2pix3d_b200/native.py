@@ -165,7 +165,8 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
     `plane_index` ([B] int32): plane set of each image; lets B views share fewer plane sets (planes batch < B).
     `out` (optional dict): contiguous buffers to write instead of fresh ones, keyed like the outputs and the debug dict
     (feat, depth, wsum, weights_final, perm, weights_coarse, depths_fine, inds); each may be longer than the launch needs,
-    and the launch writes only its leading elements."""
+    and the launch writes only its leading elements. `out['depths_sorted']` additionally asks for the merged depths in sorted
+    order, [B,R,Sc+Sf] (what render_bwd recomputes a ray from); no other output changes when it is given."""
     Bp, _, H, W, C = planes_nhwc.shape
     B = ray_origins.shape[0]
     if plane_index is None and Bp != B:
@@ -242,6 +243,8 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
             dbg['inds'] = alloc('inds', (B, R, Sf), torch.int32)
             a.dbg_weights_coarse = dbg['weights_coarse'].data_ptr()
             a.dbg_depths_fine, a.dbg_inds = dbg['depths_fine'].data_ptr(), dbg['inds'].data_ptr()
+    if 'depths_sorted' in out:
+        a.out_depths_sorted = alloc('depths_sorted', (B, R, Sc + Sf), torch.float32).data_ptr()
     a.workspace = ws.data_ptr()
     if strided:
         a.plane_strides[0], a.plane_strides[1], a.plane_strides[2] = st_img, st_plane, st_pix
@@ -275,6 +278,57 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
     if debug:
         return feat, depth, wsum, dbg
     return feat, depth, wsum
+
+
+def render_bwd(planes_nhwc, params, sigma_net, masks, ray_origins, ray_dirs, depths_sorted, Sc, Sf, box_warp, g_feat, g_depth=None,
+               g_wsum=None, depth_range=None, white_back=False, want_planes=True, want_params=True):
+    """First-order backward of render_fwd (p3d_render_bwd): recomputes every ray from the planes [B,3,H,W,32], its sorted
+    depths [B,R,Sc+Sf] (render_fwd's out['depths_sorted']) and the decoder's EFFECTIVE parameters `params` (per net
+    (w1, b1, w2, b2) with the gains applied, as _effective_fc forms them). g_feat [B,R,C]; g_depth / g_wsum [B,R(,1)] or None;
+    depth_range: device [2] = (min, max) of all depths, needed with g_depth. Returns (dL/dplanes [B,3,H,W,32] or None,
+    dL/dparams [n_nets,4257] = w1 | b1 | w2 | b2 per net, or None)."""
+    B, _, H, W, C = planes_nhwc.shape
+    assert C == 32 and planes_nhwc.dtype == torch.float32
+    p = _f32c(planes_nhwc)
+    R = ray_origins.shape[1]
+    o, d = _f32c(ray_origins), _f32c(ray_dirs)
+    ds = _f32c(depths_sorted).reshape(B, R, Sc + Sf)
+    gf = _f32c(g_feat).reshape(B, R, -1)
+    n_nets = len(params)
+    assert gf.shape[-1] == 32 * n_nets
+    keep = [p, o, d, ds, gf]
+    a = _lib.RenderBwdArgs()
+    a.planes_nhwc, a.ray_origins, a.ray_dirs, a.depths_sorted = p.data_ptr(), o.data_ptr(), d.data_ptr(), ds.data_ptr()
+    for i, net in enumerate(params):
+        w1, b1, w2, b2 = (_f32c(t.detach()) for t in net)
+        keep += [w1, b1, w2, b2]
+        a.w1[i], a.b1[i], a.w2[i], a.b2[i] = w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr()
+        a.sigmoid_mask[i] = masks[i]
+    a.n_nets, a.sigma_net = n_nets, sigma_net
+    a.B, a.R, a.H, a.W, a.Sc, a.Sf = B, R, H, W, Sc, Sf
+    a.coord_scale = 2.0 / float(box_warp)
+    a.white_back = 1 if white_back else 0
+    a.g_feat = gf.data_ptr()
+    for name, t in (('g_depth', g_depth), ('g_wsum', g_wsum), ('depth_range', depth_range)):
+        if t is not None:
+            t = _f32c(t)
+            keep.append(t)
+            setattr(a, name, t.data_ptr())
+    dev = p.device
+    g_planes = torch.empty(B, 3, H, W, 32, device=dev, dtype=torch.float32) if want_planes else None
+    g_params = None
+    with torch.cuda.device(dev):
+        if want_params:
+            g_params = torch.empty(n_nets, DECODER_PARAM_FLOATS, device=dev, dtype=torch.float32)
+            nws = _lib.lib().p3d_render_bwd_workspace_floats(n_nets)
+            ws = torch.empty(nws, device=dev, dtype=torch.float32)
+            a.g_params, a.workspace, a.workspace_floats = g_params.data_ptr(), ws.data_ptr(), nws
+        if want_planes:
+            a.g_planes_nhwc = g_planes.data_ptr()
+        st = _lib.lib().p3d_render_bwd(ctypes.byref(a), _lib.stream_ptr())
+    _lib.check(st, 'p3d_render_bwd')
+    _lib.bump(1 + (n_nets if want_params else 0))
+    return g_planes, g_params
 
 
 def run_model(planes_nhwc, dec, coords, box_warp, impl=None, sigma_only=False):

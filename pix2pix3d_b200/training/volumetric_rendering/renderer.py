@@ -2,11 +2,11 @@
 
 Mirror of the reference's training/volumetric_rendering/renderer.py: `generate_planes` (:23),
 `project_onto_planes` (:39), `sample_from_planes` (:55), `ImportanceRenderer` (:82-253) keep their signatures.
-On CUDA, when no gradient is requested, `ImportanceRenderer.forward` is ONE persistent kernel
-(`p3d_render_fwd`, pix2pix3d_b200/csrc/render.cu) fed with the same two random tensors the reference draws
-(stratified jitter, importance u), in the same order, so the RNG stream is consumed identically. Anything the
-fused kernel does not cover (gradients, density noise, unknown decoders) takes the stage-by-stage formulation
-below, which is also what CPU tensors use.
+On CUDA, `ImportanceRenderer.forward` is ONE persistent kernel (`p3d_render_fwd`, pix2pix3d_b200/csrc/render.cu) fed with
+the same two random tensors the reference draws (stratified jitter, importance u), in the same order, so the RNG stream is
+consumed identically. When the planes or the decoder require grad, the same launch runs under `_FusedRender`, whose backward
+is one recompute kernel (`p3d_render_bwd`, csrc/render_fused_bwd.cu). Anything the fused kernels do not cover (density noise,
+rays that require grad, unknown decoders) takes the stage-by-stage formulation below, which is also what CPU tensors use.
 """
 import torch
 
@@ -46,7 +46,7 @@ def sample_from_planes(plane_axes, plane_features, coordinates, mode='bilinear',
     feats = plane_features.reshape(n * n_planes, c, h, w)
     coords = (2 / box_warp) * coordinates
     grid = project_onto_planes(plane_axes, coords).unsqueeze(1)
-    out = torch.nn.functional.grid_sample(feats, grid.float(), mode=mode, padding_mode=padding_mode, align_corners=False)
+    out = torch.nn.functional.grid_sample(feats, grid.to(feats.dtype), mode=mode, padding_mode=padding_mode, align_corners=False)
     return out.permute(0, 3, 2, 1).reshape(n, n_planes, m, c)
 
 
@@ -84,6 +84,68 @@ def sample_from_3dgrid(grid, coordinates):
 _DEFAULT_AXES = generate_planes()
 
 
+# the gradient-requiring fused path (_FusedRender); tests switch it off to compare against the staged chain
+fused_grad = True
+
+
+class _FusedRender(torch.autograd.Function):
+    """ImportanceRenderer.forward on the fused kernels, differentiable to first order w.r.t. the planes and the decoder's
+    effective parameters (`params`: w1, b1, w2, b2 per net with the gains applied, so autograd carries the gains on to the
+    module parameters as native.decoder_mlp does). Saves only the channels-last planes and the sorted sample depths; the
+    backward (p3d_render_bwd) recomputes each ray from them."""
+
+    @staticmethod
+    def forward(ctx, planes, call, *params):
+        planes_cl = native.planes_to_channels_last(planes.detach())
+        b, r = call['ray_origins'].shape[:2]
+        depths_sorted = torch.empty(b, r, call['Sc'] + call['Sf'], device=planes.device, dtype=torch.float32)
+        feat, depth, wsum = native.render_fwd(planes_cl, call['dec'], call['ray_origins'], call['ray_directions'],
+                                              call['depths_coarse'], call['u'], call['box_warp'], white_back=call['white_back'],
+                                              out={'depths_sorted': depths_sorted}, **call['kw'])
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(planes_cl, depths_sorted, call['ray_origins'], call['ray_directions'], *params)
+        ctx.call = {k: call[k] for k in ('sigma_net', 'masks', 'Sc', 'Sf', 'box_warp', 'white_back')}
+        ctx.n_params = len(params)
+        ctx.plane_shape = tuple(planes.shape)
+        return feat, depth, wsum
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_feat, g_depth, g_wsum):
+        from ... import tcconv
+        planes_cl, depths_sorted, o, d, *flat = ctx.saved_tensors
+        c = ctx.call
+        n_nets = ctx.n_params // 4
+        none = (None,) * (2 + ctx.n_params)
+        if g_feat is None and g_depth is None and g_wsum is None:
+            return none
+        b, r = o.shape[:2]
+        if g_feat is None:
+            g_feat = torch.zeros(b, r, 32 * n_nets, device=o.device, dtype=torch.float32)
+        rng = None
+        if g_depth is not None:
+            lo, hi = torch.aminmax(depths_sorted)               # the clamp range of the depth output (as _RayMarch.backward)
+            rng = torch.stack([lo, hi])
+        want_planes = ctx.needs_input_grad[0]
+        want_params = any(ctx.needs_input_grad[2:])
+        if not (want_planes or want_params):
+            return none
+        params = [flat[4 * i:4 * i + 4] for i in range(n_nets)]
+        g_cl, g_par = native.render_bwd(planes_cl, params, c['sigma_net'], c['masks'], o, d, depths_sorted, c['Sc'], c['Sf'],
+                                        c['box_warp'], g_feat, g_depth, g_wsum, rng, white_back=c['white_back'],
+                                        want_planes=want_planes, want_params=want_params)
+        g_planes = None
+        if g_cl is not None:
+            n, p, ch, h, w = ctx.plane_shape
+            g_planes = tcconv.nhwc_to_nchw_f32(g_cl.view(n * p, h, w, ch)).view(n, p, ch, h, w)
+        grads = [None] * ctx.n_params
+        if g_par is not None:
+            for i in range(n_nets):
+                gw1, gb1, gw2, gb2 = torch.split(g_par[i], [64 * 32, 64, 33 * 64, 33])
+                grads[4 * i:4 * i + 4] = [gw1.view(64, 32), gb1, gw2.view(33, 64), gb2]
+        return (g_planes, None, *grads)
+
+
 def _is_default_axes(axes):
     return tuple(axes.shape) == (3, 3, 3) and bool(torch.equal(axes.detach().cpu(), _DEFAULT_AXES))
 
@@ -114,7 +176,8 @@ class ImportanceRenderer(torch.nn.Module):
         else:
             ray_start, ray_end = opts['ray_start'], opts['ray_end']
 
-        fused = planes_channels_last is not None or self._fusable(planes, decoder, ray_origins, ray_directions, opts)
+        grad_fused = planes_channels_last is None and self._fusable_grad(planes, decoder, ray_origins, ray_directions, opts)
+        fused = planes_channels_last is not None or grad_fused or self._fusable(planes, decoder, ray_origins, ray_directions, opts)
         if fused:
             b, r = ray_origins.shape[:2]
             dev = ray_origins.device
@@ -134,6 +197,15 @@ class ImportanceRenderer(torch.nn.Module):
                     kw = dict(depths_coarse=None, stratified=dict(jitter=jitter, table=table, delta=(ray_end - ray_start) / (n_c - 1)))
             u = torch.rand(b * r, n_importance, device=dev) if n_importance > 0 else None
             dec = native.pack_decoder(decoder)
+            if grad_fused:
+                nets, sigma_net, masks = native.describe_decoder(decoder)
+                params = []
+                for net in nets:
+                    params += [*native._effective_fc(net[0]), *native._effective_fc(net[2])]
+                call = dict(dec=dec, ray_origins=ray_origins, ray_directions=ray_directions, depths_coarse=kw.pop('depths_coarse'),
+                            u=u, box_warp=opts['box_warp'], white_back=bool(opts.get('white_back', False)), kw=kw,
+                            sigma_net=sigma_net, masks=masks, Sc=n_c, Sf=n_importance)
+                return _FusedRender.apply(planes, call, *params)
             planes_cl = planes_channels_last if planes_channels_last is not None else native.planes_to_channels_last(planes)
             return native.render_fwd(planes_cl, dec, ray_origins, ray_directions, kw.pop('depths_coarse'), u, opts['box_warp'],
                                      white_back=bool(opts.get('white_back', False)), plane_index=plane_index, **kw)
@@ -178,6 +250,20 @@ class ImportanceRenderer(torch.nn.Module):
         if opts['depth_resolution_importance'] > 0 and opts['depth_resolution'] < 4:
             return False
         return native.describe_decoder(decoder) is not None
+
+    def _fusable_grad(self, planes, decoder, ray_origins, ray_directions, opts):
+        """True when a gradient-requiring call can run on _FusedRender: gradients reach the planes or the decoder only (the
+        rays carry none), CUDA fp32 [B,3,32,H,W] planes of the rays' batch, and options the fused kernels cover."""
+        if not (fused_grad and torch.is_grad_enabled()):
+            return False
+        if not (planes.requires_grad or any(p.requires_grad for p in decoder.parameters())):
+            return False
+        if ray_origins.requires_grad or ray_directions.requires_grad:
+            return False
+        if (planes.device.type != 'cuda' or planes.dtype != torch.float32 or planes.ndim != 5 or planes.shape[1] != 3
+                or planes.shape[2] != 32 or planes.shape[0] != ray_origins.shape[0]):
+            return False
+        return self.fusable_options(decoder, opts) and opts['depth_resolution'] + opts['depth_resolution_importance'] >= 2
 
     def _forward_staged(self, planes, decoder, ray_origins, ray_directions, depths_coarse, n_importance, opts):
         b, r, s, _ = depths_coarse.shape
