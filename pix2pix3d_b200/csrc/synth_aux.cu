@@ -759,6 +759,7 @@ extern "C" int p3d_modulate_weights(const float* weight, const float* styles, in
                                     float out_scale, int planes, void* out, p3d_stream_t stream) {
     if (!weight || !styles || !out || B <= 0 || Cout <= 0 || Cin <= 0 || ktaps <= 0) return P3D_BAD_ARG;
     if (Cout_padded < Cout || cin_offset < 0 || Cin_padded < Cin + cin_offset || planes < 1 || planes > 2 || B > 65535) return P3D_BAD_ARG;
+    if (Cin_padded % 8 == 0 && ((uintptr_t)out & 15) != 0) return P3D_BAD_ARG;      // 16-byte row stores (vec8)
     const size_t smem = ((size_t)ktaps * (Cin + 1) + Cin) * sizeof(float);
     if (smem > 200 * 1024) return P3D_UNSUPPORTED;
     if (smem > 48 * 1024)
@@ -781,6 +782,7 @@ extern "C" int p3d_modulate_weights_t(const float* weight_t, const float* wsq, c
                                       float out_scale, int planes, void* out, p3d_stream_t stream) {
     if (!weight_t || !wsq || !styles || !out || B <= 0 || Cout <= 0 || Cin <= 0 || ktaps <= 0) return P3D_BAD_ARG;
     if (Cout_padded < Cout || cin_offset < 0 || Cin_padded < Cin + cin_offset || planes < 1 || planes > 2) return P3D_BAD_ARG;
+    if ((((uintptr_t)out | (uintptr_t)weight_t) & 15) != 0) return P3D_BAD_ARG;     // 16-byte stores, float4 weight loads
     const int nchunk = Cin_padded / 8;
     if (Cin_padded % 8 != 0 || nchunk > 256 || 256 % nchunk != 0) return P3D_UNSUPPORTED;
     modulate_weights_t_kernel<<<Cout_padded, 256, 0, (cudaStream_t)stream>>>(weight_t, wsq, styles, Cout, Cin, ktaps, Cout_padded,
@@ -793,6 +795,7 @@ extern "C" int p3d_modulate_weights_t(const float* weight_t, const float* wsq, c
 extern "C" int p3d_modulate_weights_batch(const p3d_modw_desc_t* descs_dev, const int32_t* block_layer_dev, int n_blocks,
                                           const float* styles_base, void* out_base, int B, p3d_stream_t stream) {
     if (!descs_dev || !block_layer_dev || !styles_base || !out_base || n_blocks <= 0 || B <= 0) return P3D_BAD_ARG;
+    if (((uintptr_t)out_base & 15) != 0) return P3D_BAD_ARG;                         // 16-byte stores (layer offsets are 128-byte multiples)
     modulate_weights_batch_kernel<<<n_blocks, 256, 0, (cudaStream_t)stream>>>(descs_dev, block_layer_dev, styles_base,
                                                                               (__half*)out_base, B);
     P3D_LAUNCH_CHECK();
@@ -859,6 +862,7 @@ static int fir_act_nhwc_impl(bool split_in, const void* x, int in_dtype, const f
     const int es = in_dtype == P3D_F32 ? 4 : 2, cb = 128 / es;
     if (C % cb) return P3D_UNSUPPORTED;
     if (((uintptr_t)x & 15) != 0) return P3D_BAD_ARG;
+    if (((uintptr_t)y & (es == 2 ? 15 : 7)) != 0) return P3D_BAD_ARG;            // 16-byte (fp16 input) or 8-byte output stores
     CUtensorMap tm;
     {
         uint64_t dims[4] = {(uint64_t)C, (uint64_t)inW, (uint64_t)inH, (uint64_t)B * (split_in ? 2 : 1)};   // lo plane = images B..2B-1

@@ -93,8 +93,10 @@ def _pad_vec(v, n):
     return out
 
 
-def _bias(layer, n):
-    return _cached(layer, ('bias', n), [layer.bias], lambda: _pad_vec(layer.bias, n))
+def _bias(layer, n, half=False):
+    """The layer's bias padded to n channels, in fp32. `half`: rounded to fp16 first, as the reference's fp16 layers apply it
+    (`bias_act(x, self.bias.to(x.dtype))`, networks_stylegan2.py:331, :358)."""
+    return _cached(layer, ('bias', n, half), [layer.bias], lambda: _pad_vec(layer.bias.detach().half() if half else layer.bias, n))
 
 
 def _prepared(layer):
@@ -292,7 +294,7 @@ def synthesis_layer(layer, x, styles, noise_mode, split, gain=1.0, cin_offset=0,
         wk = tcconv.modulate_weights(layer.weight, styles, demodulate=True, planes=planes, cin_padded=cin_p, cin_offset=cin_offset,
                                      prepared=_prepared(layer))
     noise = _noise(layer, noise_mode, b)
-    bias = _bias(layer, cout_p)
+    bias = _bias(layer, cout_p, half=not split)
     act_gain = layer.act_gain * gain
     clamp = float(layer.conv_clamp * gain) if layer.conv_clamp is not None else -1.0
     dev = x.device
@@ -306,7 +308,7 @@ def synthesis_layer(layer, x, styles, noise_mode, split, gain=1.0, cin_offset=0,
                 return None
             y = torch.empty(1, b, h, w, cout, device=dev, dtype=torch.float16)       # never written (rgb_skip_x); the ABI wants a buffer
             image = torch.empty(b, ci, h, w, device=dev, dtype=torch.float32)
-            rgb = dict(w=st.wk[0], bias=_bias(torgb, ci), prev=rgb_tail['prev'].contiguous(), filter=rgb_tail['filter'], out=image,
+            rgb = dict(w=st.wk[0], bias=_bias(torgb, ci, half=True), prev=rgb_tail['prev'].contiguous(), filter=rgb_tail['filter'], out=image,
                        clamp=float(torgb.conv_clamp) if torgb.conv_clamp is not None else -1.0, skip_x=True)
             ok = tcconv.conv_gemm_try(x, wk, cout, tcconv.TAPS_3X3, (h, w), y[0], out_mode=0, split=False, bias=bias, noise=noise, act=3,
                                       alpha=0.2, gain=act_gain, clamp=clamp, rgb=rgb)
@@ -344,7 +346,7 @@ def torgb_layer(layer, x, styles, img, split, upsample_filter=None, final_nchw=F
         wk = tcconv.modulate_weights(layer.weight, styles, demodulate=False, pre_scale=layer.weight_gain, planes=planes,
                                      cin_padded=x.shape[-1], prepared=_prepared(layer))
     h, w = x.shape[2], x.shape[3]
-    bias = _bias(layer, cout)
+    bias = _bias(layer, cout, half=not split)
     clamp = float(layer.conv_clamp) if layer.conv_clamp is not None else -1.0
     if upsample_filter is not None and img is not None:
         assert img.shape[1] * 2 == h and img.shape[2] * 2 == w and img.shape[3] == cout

@@ -42,13 +42,21 @@ def pad_to(n, m):
     return (n + m - 1) // m * m
 
 
-def to_nhwc_f16(x, c_padded=None, planes=1):
-    """NCHW fp32/fp16 -> [planes,N,H,W,Cp] fp16."""
+def _out(out, shape, like, dtype):
+    """The caller's output tensor (checked against the launch's shape), or a new one."""
+    if out is None:
+        return torch.empty(shape, device=like.device, dtype=dtype)
+    assert tuple(out.shape) == tuple(shape) and out.dtype == dtype and out.is_contiguous() and out.device == like.device
+    return out
+
+
+def to_nhwc_f16(x, c_padded=None, planes=1, out=None):
+    """NCHW fp32/fp16 -> [planes,N,H,W,Cp] fp16 (into `out` when given)."""
     assert x.is_cuda and x.ndim == 4
     x = x.contiguous()
     n, c, h, w = x.shape
     cp = c_padded or c
-    out = torch.empty(planes, n, h, w, cp, device=x.device, dtype=torch.float16)
+    out = _out(out, (planes, n, h, w, cp), x, torch.float16)
     with torch.cuda.device(x.device):
         st = _lib.lib().p3d_nchw_to_nhwc_f16(_lib.ptr(x), _lib.DTYPE_CODE[x.dtype], n, c, h, w, cp, planes, _lib.ptr(out),
                                              _lib.stream_ptr())
@@ -57,12 +65,12 @@ def to_nhwc_f16(x, c_padded=None, planes=1):
     return out
 
 
-def nhwc_to_nchw_f32(x, channels=None, c_offset=0):
-    """[N,H,W,Cs] fp32 -> [N,channels,H,W] fp32 taking channels [c_offset, c_offset+channels)."""
+def nhwc_to_nchw_f32(x, channels=None, c_offset=0, out=None):
+    """[N,H,W,Cs] fp32 -> [N,channels,H,W] fp32 taking channels [c_offset, c_offset+channels) (into `out` when given)."""
     assert x.is_cuda and x.dtype == torch.float32 and x.ndim == 4 and x.is_contiguous()
     n, h, w, cs = x.shape
     c = channels or cs
-    out = torch.empty(n, c, h, w, device=x.device, dtype=torch.float32)
+    out = _out(out, (n, c, h, w), x, torch.float32)
     with torch.cuda.device(x.device):
         st = _lib.lib().p3d_nhwc_to_nchw_f32(_lib.ptr(x), n, c, h, w, cs, c_offset, _lib.ptr(out), _lib.stream_ptr())
     _lib.check(st, 'p3d_nhwc_to_nchw_f32')
@@ -129,11 +137,12 @@ def modulate_weights_batch(descs_dev, block_layer_dev, n_blocks, styles_flat, ou
     _lib.bump()
 
 
-def affine_batch(ws, weight, bias, meta, out_numel):
-    """ws [B,num_ws,w_dim] fp32; weight [rows,w_dim] (gains applied), bias [rows], meta int32 [rows,4] -> flat fp32 buffer."""
+def affine_batch(ws, weight, bias, meta, out_numel, out=None):
+    """ws [B,num_ws,w_dim] fp32; weight [rows,w_dim] (gains applied), bias [rows], meta int32 [rows,4] -> flat fp32 buffer
+    (`out` when given)."""
     ws = ws.detach().float().contiguous()
     b, num_ws, w_dim = ws.shape
-    out = torch.empty(out_numel, device=ws.device, dtype=torch.float32)
+    out = _out(out, (out_numel,), ws, torch.float32)
     with torch.cuda.device(ws.device):
         st = _lib.lib().p3d_affine_batch(_lib.ptr(ws), _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(meta), _lib.ptr(out), b, num_ws, w_dim,
                                          weight.shape[0], _lib.stream_ptr())
@@ -324,8 +333,10 @@ def separable_factors(f):
     return hit[1]
 
 
-def fir_act_nhwc(x, f, noise, bias, out_planes, out_hw, pad0=(1, 1), fir_gain=4.0, act=3, alpha=0.2, act_gain=1.0, clamp=-1.0):
-    """x [B,inH,inW,C] fp32/fp16 NHWC, or a split fp16 pair [2,B,inH,inW,C] -> [out_planes,B,outH,outW,C] fp16."""
+def fir_act_nhwc(x, f, noise, bias, out_planes, out_hw, pad0=(1, 1), fir_gain=4.0, act=3, alpha=0.2, act_gain=1.0, clamp=-1.0,
+                 out=None):
+    """x [B,inH,inW,C] fp32/fp16 NHWC, or a split fp16 pair [2,B,inH,inW,C] -> [out_planes,B,outH,outW,C] fp16 (into `out`
+    when given)."""
     split_in = x.ndim == 5
     if split_in:
         assert x.shape[0] == 2 and x.dtype == torch.float16 and x.is_contiguous()
@@ -333,7 +344,7 @@ def fir_act_nhwc(x, f, noise, bias, out_planes, out_hw, pad0=(1, 1), fir_gain=4.
     else:
         b, ih, iw, c = x.shape
     oh, ow = out_hw
-    y = torch.empty(out_planes, b, oh, ow, c, device=x.device, dtype=torch.float16)
+    y = _out(out, (out_planes, b, oh, ow, c), x, torch.float16)
     nbs = 0 if (noise is None or noise.ndim == 2) else oh * ow          # per-sample noise images (noise_mode='random')
     if noise is not None:
         assert noise.is_contiguous() and noise.dtype == torch.float32 and noise.shape[-2:] == (oh, ow)
@@ -356,9 +367,10 @@ def fir_act_nhwc(x, f, noise, bias, out_planes, out_hw, pad0=(1, 1), fir_gain=4.
     return y
 
 
-def upsample2x_nhwc(x, f):
+def upsample2x_nhwc(x, f, out=None):
+    """upfirdn2d.upsample2d(x, f) on fp32 NHWC [B,H,W,C] -> [B,2H,2W,C] (into `out` when given)."""
     b, h, w, c = x.shape
-    y = torch.empty(b, 2 * h, 2 * w, c, device=x.device, dtype=torch.float32)
+    y = _out(out, (b, 2 * h, 2 * w, c), x, torch.float32)
     with torch.cuda.device(x.device):
         st = _lib.lib().p3d_upsample2x_nhwc(_lib.ptr(x), _lib.ptr(f), _lib.ptr(y), b, h, w, c, _lib.stream_ptr())
     _lib.check(st, 'p3d_upsample2x_nhwc')
