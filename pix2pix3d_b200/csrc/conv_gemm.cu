@@ -14,6 +14,9 @@
 // * Persistent ping-pong: warpgroup 0 = TMA producer, warpgroups 1 and 2 = consumers that own alternate tiles (wgmma, then
 //   the epilogue: scale/noise/bias/activation/clamp -> NHWC store), so one tile's epilogue runs under the next tile's MMAs.
 //   mbarrier ring of smem stages shared by the consumers.
+// * Two epilogues, chosen per launch by the host: fp16 NHWC outputs are computed on the accumulator fragments and leave as
+//   fp16 tiles through TMA stores (conv_epilogue_tma); fp32 outputs, the resnet skip, the ToRGB tail and split-K partials
+//   are staged through shared memory as fp32 so that a thread owns one pixel (conv_store_chunk).
 // * A launch may carry up to four PHASES (ConvPhase: tap subset, grid, output offset): the four parities of a stride-2
 //   transposed 3x3 convolution run as one launch (p3d_conv_gemm_phases).
 // * The kernel can also evaluate the NEXT layer's 1x1 ToRGB + skip on the outputs it holds (rgb_* arguments): the last
@@ -75,14 +78,21 @@ struct ConvKernelArgs {
     const __half* rgb_w; const float* rgb_bias; const float* rgb_prev; const float* rgb_f; float* rgb_out;
     int rgb_cout, rgb_w_rows, rgb_skip_x;
     float rgb_clamp, rgb_acc_scale;
+    int tma_epi;                      // epilogue on the accumulator fragments, fp16 tiles stored by TMA (ConvOutMaps)
 };
 
-// phase that owns tile `t` of the launch's tile order (phases are consecutive ranges starting at ph[q].t0)
-__device__ __forceinline__ ConvPhase conv_phase_of(const ConvKernelArgs& a, int t) {
-    ConvPhase P = a.ph[0];
+// Output tensor maps of a tma_epi launch, per phase: the phase's output grid as a 4-D tensor {Cout, gW, gH, B} of fp16 (y and
+// the lo plane of out_mode 1), box {64 channels, BW, BH, 1} with a 128-byte swizzle.
+struct ConvOutMaps {
+    CUtensorMap y[4], y_lo[4];
+};
+
+// index of the phase that owns tile `t` of the launch's tile order (phases are consecutive ranges starting at ph[q].t0)
+__device__ __forceinline__ int conv_phase_of(const ConvKernelArgs& a, int t) {
+    int P = 0;
 #pragma unroll
     for (int q = 1; q < 4; ++q)
-        if (q < a.n_phases && t >= a.ph[q].t0) P = a.ph[q];
+        if (q < a.n_phases && t >= a.ph[q].t0) P = q;
     return P;
 }
 
@@ -274,11 +284,13 @@ __device__ __forceinline__ void conv_store_chunk(const ConvKernelArgs& a, uint32
 constexpr int kConvThreads = 384;
 constexpr int kStageStride = 36;                  // floats per staged pixel row: a 32-channel chunk + 4 (conflict-free rows)
 constexpr int kEpiFloats = kBM * kStageStride + 2 * 128 + 8 * 128;     // per consumer: staging, scale, bias, ToRGB weights
+static_assert(kBM * kStageStride * 4 >= kBM * 128 && (kBM * kStageStride * 4) % 1024 == 0 && (kEpiFloats * 4) % 1024 == 0,
+              "the fp16 tile of tma_epi fits the staging area, and both per-consumer areas are 1024-byte aligned");
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;                  // 128 x 40 + 256 x 232 <= 64 K registers
 
 struct ConvUnit {
     ConvPhase P;
-    int tx, ty, tile_n, b, ksplit, k_begin, total_k;
+    int q, tx, ty, tile_n, b, ksplit, k_begin, total_k;     // q: index of the phase P
 };
 
 // work unit u of the launch: u = ((b * splits + ksplit) * tiles_n + tile_n) * tiles_m + (spatial tile of the phases)
@@ -289,7 +301,11 @@ __device__ __forceinline__ ConvUnit conv_unit(const ConvKernelArgs& a, int u) {
     const int z = r / a.tiles_n;
     U.b = z / a.splits;
     U.ksplit = z - U.b * a.splits;
-    U.P = conv_phase_of(a, t);
+    U.q = conv_phase_of(a, t);
+    U.P = a.ph[0];
+#pragma unroll
+    for (int q = 1; q < 4; ++q)
+        if (q == U.q) U.P = a.ph[q];
     const int tile_m = t - U.P.t0;
     U.ty = tile_m / U.P.tiles_x;
     U.tx = tile_m - U.ty * U.P.tiles_x;
@@ -299,18 +315,180 @@ __device__ __forceinline__ ConvUnit conv_unit(const ConvKernelArgs& a, int u) {
     return U;
 }
 
+// Fused ToRGB of one pixel: out = upsample2d(prev)[b, Y, X, :] + round16(clamp(dot * scale + bias)), written NCHW (lanes =
+// consecutive X)
+__device__ __forceinline__ void conv_rgb_tail(const ConvKernelArgs& a, const float (&dot)[8], int b, int Y, int X) {
+    const int ph = a.oH >> 1, pw = a.oW >> 1, C = a.rgb_cout;
+    const int iy = Y >> 1, py = Y & 1, ix = X >> 1, px = X & 1;
+    float w4[2][2];
+    const float* pp[2][2];
+#pragma unroll
+    for (int aa = 0; aa < 2; ++aa)
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc) {
+            const int ry = iy - 1 + py + aa, rx = ix - 1 + px + cc;
+            const bool ok = ry >= 0 && ry < ph && rx >= 0 && rx < pw;
+            w4[aa][cc] = ok ? __ldg(a.rgb_f + (3 - (py + 2 * aa)) * 4 + (3 - (px + 2 * cc))) * 4.f : 0.f;
+            pp[aa][cc] = a.rgb_prev + (((size_t)b * ph + (ok ? ry : 0)) * pw + (ok ? rx : 0)) * C;
+        }
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        if (c < C) {
+            float up = 0.f;
+#pragma unroll
+            for (int aa = 0; aa < 2; ++aa)
+#pragma unroll
+                for (int cc = 0; cc < 2; ++cc) up = fmaf(w4[aa][cc], __ldg(pp[aa][cc] + c), up);
+            float x = fmaf(dot[c], a.rgb_acc_scale, a.rgb_bias ? __ldg(a.rgb_bias + c) : 0.f);
+            if (a.rgb_clamp >= 0.f) x = fminf(fmaxf(x, -a.rgb_clamp), a.rgb_clamp);
+            x = __half2float(__float2half_rn(x));
+            a.rgb_out[(((size_t)b * C + c) * a.oH + Y) * a.oW + X] = up + x;
+        }
+    }
+}
+
+// Epilogue of a tma_epi launch (fp16 NHWC outputs, see conv_launch), applied to the accumulator fragments in registers. Thread
+// (warp wq, lane l) of the warpgroup holds pixels r0 = 16 wq + l/4 and r0 + 8 (acc0), r0 + 64 and r0 + 72 (acc1) x channels
+// 8i + 2(l%4) + {0,1}. Each 64-channel half of the tile (and each plane, for hi/lo outputs) is packed to fp16 with stmatrix
+// into the warpgroup's [128 px][64 ch] tile, 128-byte swizzled as a TMA box {64, BW, BH, 1} lays it out, and one thread
+// stores it with TMA; the store clips ragged tiles and channels past Cout. The fused ToRGB reads each pixel's row of the
+// tile back, so its dot products see the same fp16 values in the same order as the staged epilogue's.
+template <int kAct, bool kClamp, int kBN>
+__device__ __forceinline__ void conv_epilogue_tma(const ConvKernelArgs& a, const ConvOutMaps& om, const ConvUnit& U, uint8_t* tile,
+                                                  const float* s_scale, const float* s_bias, const float* s_rgbw,
+                                                  const float (&acc0)[kBN / 2], const float (&acc1)[kBN / 2], int cw) {
+    const int m = threadIdx.x & 127, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const ConvPhase& P = U.P;
+    const int b = U.b, n0 = U.tile_n * kBN;
+    const float alpha = a.alpha, post_gain = a.post_gain, clampv = a.clamp;
+    // noise of the thread's pixels r0 + {0, 8, 64, 72}, read once per unit
+    float nz[4];
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+        const int r = wq * 16 + (lane >> 2) + 8 * (p & 1) + 64 * (p >> 1);
+        const int gy = U.ty * a.BH + r / a.BW, gx = U.tx * a.BW + r % a.BW;
+        nz[p] = (a.noise && gy < P.gH && gx < P.gW)
+                    ? __ldg(a.noise + (size_t)b * a.noise_bstride + (size_t)(gy * a.sy + P.oy) * a.oW + gx * a.sx + P.ox) * a.pre_gain
+                    : 0.f;
+    }
+    // stmatrix addresses: lane l gives row l % 8 of matrix l / 8 = (8-row half (l / 8) % 2, column group l / 16 of the pair)
+    const uint32_t tile_s = tc::smem_u32(tile);
+    const int st_row = wq * 16 + 8 * ((lane >> 3) & 1) + (lane & 7), st_grp = lane >> 4;
+    const int cq = 2 * (lane & 3);
+    const bool hilo = a.out_mode == 1;
+    const bool store = !a.rgb_w || !a.rgb_skip_x;
+    // before the tile is written: the last store has read it and every thread is done with it (constants visible)
+    auto tile_acquire = [&]() {
+        if (m == 0) tc::bulk_wait_read<0>();
+        tc::named_bar_sync(3 + cw, 128);
+    };
+    // after it is written: visible to the TMA unit and to the warpgroup; one thread stores the box at channel c
+    auto tile_release = [&](const CUtensorMap* tm, int c) {
+        if (store) tc::fence_proxy_async();
+        tc::named_bar_sync(3 + cw, 128);
+        if (store && m == 0) {
+            tc::tma_store_4d(tm, tile, c, U.tx * a.BW, U.ty * a.BH, b);
+            tc::bulk_commit();
+        }
+    };
+    float dot[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) dot[c] = 0.f;
+#pragma unroll
+    for (int hf = 0; hf < kBN / 64; ++hf) {
+        const int c_half = n0 + 64 * hf;
+        if (c_half >= a.Cout) break;
+        // the fp16 values of this half (lo_plane: the hi/lo remainders) into the tile, one 8x8 matrix per column group and
+        // 8-row half of the warp's rows
+        auto write_tile = [&](bool lo_plane) {
+#pragma unroll
+            for (int i = 0; i < 8; i += 2) {                     // column groups 8 hf + i, 8 hf + i + 1
+#pragma unroll
+                for (int ah = 0; ah < 2; ++ah) {                 // acc0: rows 0-63, acc1: rows 64-127
+                    uint32_t r[4];
+#pragma unroll
+                    for (int mq = 0; mq < 4; ++mq) {             // matrix mq: rows + 8 (mq & 1), column group + (mq >> 1)
+                        const int h = mq & 1, g = 8 * hf + i + (mq >> 1);
+                        const float2 sc = *reinterpret_cast<const float2*>(s_scale + 8 * g + cq);
+                        const float2 bi = *reinterpret_cast<const float2*>(s_bias + 8 * g + cq);
+                        const float n = nz[h + 2 * ah];
+                        const float v0 = ah ? acc1[4 * g + 2 * h] : acc0[4 * g + 2 * h];
+                        const float v1 = ah ? acc1[4 * g + 2 * h + 1] : acc0[4 * g + 2 * h + 1];
+                        const float x0 = conv_epilogue_act<kAct, kClamp>(fmaf(v0, sc.x, bi.x) + n, alpha, post_gain, clampv);
+                        const float x1 = conv_epilogue_act<kAct, kClamp>(fmaf(v1, sc.y, bi.y) + n, alpha, post_gain, clampv);
+                        __half2 hv = __floats2half2_rn(x0, x1);
+                        if (lo_plane) {
+                            const float2 back = __half22float2(hv);
+                            hv = __floats2half2_rn(x0 - back.x, x1 - back.y);
+                        }
+                        r[mq] = *reinterpret_cast<const uint32_t*>(&hv);
+                    }
+                    const int row = st_row + 64 * ah, j = i + st_grp;
+                    tc::stmatrix_x4(tile_s + row * 128 + ((j ^ (row & 7)) << 4), r[0], r[1], r[2], r[3]);
+                }
+            }
+        };
+        tile_acquire();
+        write_tile(false);
+        tile_release(&om.y[U.q], c_half);
+        if (hilo) {
+            tile_acquire();
+            write_tile(true);
+            tile_release(&om.y_lo[U.q], c_half);
+        } else if (a.rgb_w) {
+            // dot products of this pixel's fp16 outputs with the ToRGB weights, channels in order (Cout % 32 == 0); a
+            // quarter-warp reads 8 rows at 8 different swizzled 16-byte columns, so without bank conflicts
+            const int nv = min(64, a.Cout - c_half);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                if (8 * j >= nv) break;
+                const uint4 t = *reinterpret_cast<const uint4*>(tile + m * 128 + ((j ^ (m & 7)) << 4));
+                const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
+                float xv[8];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&tw[e]));
+                    xv[2 * e] = f.x; xv[2 * e + 1] = f.y;
+                }
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    if (c < a.rgb_cout) {
+                        const float4* wr = reinterpret_cast<const float4*>(s_rgbw + c * 128 + 64 * hf + 8 * j);
+                        const float4 w0 = wr[0], w1 = wr[1];
+                        float acc_c = dot[c];
+                        acc_c = fmaf(xv[0], w0.x, acc_c); acc_c = fmaf(xv[1], w0.y, acc_c);
+                        acc_c = fmaf(xv[2], w0.z, acc_c); acc_c = fmaf(xv[3], w0.w, acc_c);
+                        acc_c = fmaf(xv[4], w1.x, acc_c); acc_c = fmaf(xv[5], w1.y, acc_c);
+                        acc_c = fmaf(xv[6], w1.z, acc_c); acc_c = fmaf(xv[7], w1.w, acc_c);
+                        dot[c] = acc_c;
+                    }
+                }
+            }
+        }
+    }
+    // the tile is free again (and, at the warpgroup's last unit, no store reads shared memory after the CTA exits)
+    if (m == 0) tc::bulk_wait_read<0>();
+    if (a.rgb_w) {
+        const int gy = U.ty * a.BH + m / a.BW, gx = U.tx * a.BW + m % a.BW;
+        if (gy < P.gH && gx < P.gW) conv_rgb_tail(a, dot, b, gy * a.sy + P.oy, gx * a.sx + P.ox);
+    }
+}
+
 template <int kAct, bool kClamp, int kBN>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                    const __grid_constant__ CUtensorMap tmB,
-                                                                   const ConvKernelArgs a, int n_stages) {
+                                                                   const ConvKernelArgs a, const __grid_constant__ ConvOutMaps om,
+                                                                   int n_stages) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [stages][A 16 KB][B BN*128 B] | barriers | per consumer warpgroup: [128 px][kStageStride] fp32 staging,
-    // per-channel scale, bias | fused ToRGB weights [8][128]
+    // carve: [stages][A 16 KB][B BN*128 B] | per consumer warpgroup: [128 px][kStageStride] fp32 staging (or, for tma_epi,
+    // the [128 px][64 ch] fp16 tile), per-channel scale, bias, fused ToRGB weights [8][128] | barriers. Stages and per-consumer
+    // areas are multiples of 1024 bytes, so every staging area is 1024-byte aligned (the 128-byte swizzle repeats every 1024).
     // round up inside the shared window (pointer arithmetic on smem_raw keeps the address space known to the compiler)
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t a_bytes = (uint32_t)kBM * 128, b_bytes = (uint32_t)kBN * 128;
     const uint32_t stage_bytes = a_bytes + b_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + n_stages * stage_bytes);
+    uint8_t* epi = smem + n_stages * stage_bytes;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi + 2 * kEpiFloats * sizeof(float));
     uint64_t* empty_bar = full_bar + kMaxStages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -354,7 +532,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     // ===== consumers: warpgroup cw takes units i = cw, cw + 2, ... of this CTA's list =====
     const int cw = wg - 1, wq = warp & 3;
     const int m = threadIdx.x & 127;              // epilogue: thread = pixel (tile row m)
-    float* stg = reinterpret_cast<float*>(empty_bar + kMaxStages) + cw * kEpiFloats;
+    float* stg = reinterpret_cast<float*>(epi) + cw * kEpiFloats;
     float* s_scale = stg + kBM * kStageStride;
     float* s_bias = s_scale + 128;
     float* s_rgbw = s_bias + 128;
@@ -428,6 +606,13 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
                     const int c = j >> 7, kk = j & 127;
                     s_rgbw[j] = (c < a.rgb_cout && kk < a.Cout) ? __half2float(__ldg(a.rgb_w + ((size_t)b * a.rgb_w_rows + c) * a.Cout + kk)) : 0.f;
                 }
+            }
+        }
+
+        if constexpr (kBN >= 64) {
+            if (a.tma_epi) {
+                conv_epilogue_tma<kAct, kClamp, kBN>(a, om, U, reinterpret_cast<uint8_t*>(stg), s_scale, s_bias, s_rgbw, acc0, acc1, cw);
+                continue;
             }
         }
 
@@ -510,36 +695,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
                 conv_store_chunk<kAct, kClamp>(a, v, s_scale, s_bias, c0, ch0, off, nz, vec_ok, b, Y, X);
             }
         }
-        if (a.rgb_w && pix_ok) {
-            // out = upsample2d(prev)[b, Y, X, :] + round16(clamp(dot * scale + bias)), written NCHW (lanes = consecutive X)
-            const int ph = a.oH >> 1, pw = a.oW >> 1, C = a.rgb_cout;
-            const int iy = Y >> 1, py = Y & 1, ix = X >> 1, px = X & 1;
-            float w4[2][2];
-            const float* pp[2][2];
-#pragma unroll
-            for (int aa = 0; aa < 2; ++aa)
-#pragma unroll
-                for (int cc = 0; cc < 2; ++cc) {
-                    const int ry = iy - 1 + py + aa, rx = ix - 1 + px + cc;
-                    const bool ok = ry >= 0 && ry < ph && rx >= 0 && rx < pw;
-                    w4[aa][cc] = ok ? __ldg(a.rgb_f + (3 - (py + 2 * aa)) * 4 + (3 - (px + 2 * cc))) * 4.f : 0.f;
-                    pp[aa][cc] = a.rgb_prev + (((size_t)b * ph + (ok ? ry : 0)) * pw + (ok ? rx : 0)) * C;
-                }
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                if (c < C) {
-                    float up = 0.f;
-#pragma unroll
-                    for (int aa = 0; aa < 2; ++aa)
-#pragma unroll
-                        for (int cc = 0; cc < 2; ++cc) up = fmaf(w4[aa][cc], __ldg(pp[aa][cc] + c), up);
-                    float x = fmaf(dot[c], a.rgb_acc_scale, a.rgb_bias ? __ldg(a.rgb_bias + c) : 0.f);
-                    if (a.rgb_clamp >= 0.f) x = fminf(fmaxf(x, -a.rgb_clamp), a.rgb_clamp);
-                    x = __half2float(__float2half_rn(x));
-                    a.rgb_out[(((size_t)b * C + c) * a.oH + Y) * a.oW + X] = up + x;
-                }
-            }
-        }
+        if (a.rgb_w && pix_ok) conv_rgb_tail(a, dot, b, Y, X);
     }
 }
 
@@ -779,6 +935,28 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
             }
         }
     }
+    // fp16 NHWC outputs whose 16-byte channel groups stay aligned take the epilogue on the accumulator fragments with TMA
+    // stores (conv_epilogue_tma): one output map per phase and plane, a view of the phase's grid inside the output tensor.
+    // Everything else (fp32 outputs, resnet skip, fused ToRGB tail, split-K partials, 32-channel tiles) takes the staged one.
+    ConvOutMaps om;
+    memset(&om, 0, sizeof(om));
+    a.tma_epi = 0;
+    if (p->out_mode <= 1 && !p->residual && !p->up_prev && a.splits == 1 && BN >= 64 && p->y_coff % 8 == 0 &&
+        p->y_cstride % 8 == 0 && ((((uintptr_t)p->y) | (p->out_mode == 1 ? (uintptr_t)p->y_lo : 0)) & 15) == 0) {
+        const uint64_t cs = (uint64_t)p->y_cstride * 2;
+        int rc = P3D_OK;
+        for (int q = 0; q < n_phases && rc == P3D_OK; ++q) {
+            const p3d_conv_args_t* r = phases + q;
+            const size_t off = ((size_t)r->oy * p->oW + r->ox) * p->y_cstride + p->y_coff;
+            const uint64_t dims[4] = {(uint64_t)p->Cout, (uint64_t)r->gW, (uint64_t)r->gH, (uint64_t)p->B};
+            const uint64_t str[3] = {(uint64_t)p->sx * cs, (uint64_t)p->sy * p->oW * cs, (uint64_t)p->oH * p->oW * cs};
+            const uint32_t box[4] = {64, (uint32_t)BW, (uint32_t)BH, 1};
+            rc = make_tmap_f16_sw128(&om.y[q], reinterpret_cast<const __half*>(p->y) + off, 4, dims, str, box);
+            if (rc == P3D_OK && p->out_mode == 1)
+                rc = make_tmap_f16_sw128(&om.y_lo[q], reinterpret_cast<const __half*>(p->y_lo) + off, 4, dims, str, box);
+        }
+        a.tma_epi = rc == P3D_OK;
+    }
     // persistent grid: at most one CTA per SM (the kernel's registers and shared memory allow no more) walking the work units
     // (grid.x spatial tiles x grid.y channel tiles x grid.z samples and k-splits) in the order of the one-tile-per-CTA grid
     a.B = p->B; a.tiles_m = (int)grid.x; a.tiles_n = (int)grid.y;
@@ -795,7 +973,7 @@ static int conv_launch(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t
     do {                                                                                                                      \
         P3D_CUDA_TRY(cudaFuncSetAttribute(conv_gemm_kernel<ACT, CL, BNV>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
                                           (int)smem));                                                                        \
-        conv_gemm_kernel<ACT, CL, BNV><<<n_ctas, kConvThreads, smem, (cudaStream_t)stream>>>(tmA, tmB, a, n_stages);         \
+        conv_gemm_kernel<ACT, CL, BNV><<<n_ctas, kConvThreads, smem, (cudaStream_t)stream>>>(tmA, tmB, a, om, n_stages);     \
     } while (0)
 #define P3D_LAUNCH_CONV(ACT, CL)                                                                                              \
     do {                                                                                                                      \

@@ -74,6 +74,24 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tm, ui
         ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
 }
+// shared -> global tile store; out-of-bounds elements of the box are not written. Completion is tracked per thread by bulk
+// groups: commit after the stores, then wait_read before the source buffer is overwritten or the CTA exits.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, const void* src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(tm), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+
+// Four 8x8 fp16 matrices from registers to shared memory: r[q] holds the pair (row lane/4, columns 2(lane%4) + {0,1}) of
+// matrix q, lanes 8q..8q+7 give the addresses of matrix q's rows 0..7 (16 bytes each). This is the accumulator fragment
+// layout of wgmma, so a packed 8-column group of an accumulator is one matrix.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
 
 // ---- wgmma ------------------------------------------------------------------------------------
 // K-major operand tile in shared memory, 128-byte rows, SWIZZLE_128B (what a TMA box with a 128-byte inner extent and

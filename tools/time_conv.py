@@ -3,7 +3,8 @@
     python tools/time_conv.py [--workload seg2cat_512] [--steps 12] [--warmup 3] [--json FILE]
 
 Prints one row per conv launch of a step: layer shape (B, computed grid, Cin, Cout, taps, phases, precision passes), the
-tiling the library picks for it (BN, 128-pixel tiles, k-steps per tile, split-K factor, work units), the median time over
+tiling the library picks for it (BN, 128-pixel tiles, k-steps per tile, split-K factor, work units, and which epilogue:
+`tma` on the accumulator fragments with TMA stores, or `staged` through shared memory), the median time over
 the timed steps and the executed TFLOP/s (the fp32 layers execute three fp16 passes). The tiling columns mirror the host
 rules of conv_launch in csrc/conv_gemm.cu.
 """
@@ -51,7 +52,11 @@ def tiling(phases, sms):
             s -= 1
         if s > 1 and p.splitk_scratch % 32 == 0:
             splits = s
-    return dict(BN=bn, tile=f'{bw}x{bh}', tiles=tiles_m * tiles_n, ksteps=ksteps, splits=splits, units=base * splits)
+    # epilogue: on the accumulator fragments with TMA stores, or staged through shared memory as fp32
+    tma = (p.out_mode <= 1 and not p.residual and not p.up_prev and splits == 1 and bn >= 64 and p.y_coff % 8 == 0
+           and p.y_cstride % 8 == 0 and ((p.y or 0) | ((p.y_lo or 0) if p.out_mode == 1 else 0)) % 16 == 0)
+    return dict(BN=bn, tile=f'{bw}x{bh}', tiles=tiles_m * tiles_n, ksteps=ksteps, splits=splits, units=base * splits,
+                epi='tma' if tma else 'staged')
 
 
 class _Recorder:
@@ -134,12 +139,12 @@ def main():
     name = torch.cuda.get_device_name(dev)
     print(f'# {name}, {sms} SMs; {args.workload}, median of {args.steps} eager steps after {args.warmup} warm-up')
     print(f'{"#":>3} {"B":>2} {"grid":>23} {"Cin":>4} {"Cout":>4} {"taps":>4} {"ph":>2} {"pass":>4} {"BN":>3} {"tile":>6} '
-          f'{"tiles":>6} {"k/tile":>11} {"split":>5} {"units":>6} {"us":>8} {"execTF/s":>8}')
+          f'{"tiles":>6} {"k/tile":>11} {"split":>5} {"units":>6} {"epi":>6} {"us":>8} {"execTF/s":>8}')
     for r in rows:
         ks = '/'.join(str(k) for k in r['ksteps'])
         print(f'{r["i"]:>3} {r["B"]:>2} {r["grid"]:>23} {r["Cin"]:>4} {r["Cout"]:>4}{"+rgb" if r["rgb"] else "    "}'
               f'{r["taps"]:>4} {r["phases"]:>2} {r["passes"]:>4} {r["BN"]:>3} {r["tile"]:>6} {r["tiles"]:>6} {ks:>11} '
-              f'{r["splits"]:>5} {r["units"]:>6} {r["us"]:>8.1f} {r["exec_tflops"]:>8.1f}')
+              f'{r["splits"]:>5} {r["units"]:>6} {r["epi"]:>6} {r["us"]:>8.1f} {r["exec_tflops"]:>8.1f}')
     tot_us = sum(r['us'] for r in rows)
     print(f'# {len(rows)} launches, {tot_us / 1e3:.3f} ms per step (sum of medians), '
           f'{sum(r["alg_gflop"] for r in rows) / tot_us * 1e3:.1f} TFLOP/s algorithmic, '
