@@ -182,18 +182,22 @@ int p3d_sample_from_planes_bwd(const float* grad_features, const float* coords, 
  *   gains of FullyConnectedLayer already applied by the caller, networks_stylegan2.py:111-119; Softplus(beta 1, threshold 20))
  *   out_sigma [N*M] = o[0];  out_rgb [N*M,32][k] = bit k of sigmoid_mask ? sigmoid(o[1+k]) * 1.002 - 0.001 : o[1+k].
  * out_pre (optional, [N*M,64]): the hidden pre-activations w1 x + b1, which p3d_decoder_mlp_bwd consumes (pass NULL when no
- * gradient will be taken). One launch instead of mean + addmm + softplus + addmm + slices + sigmoid + cat. */
+ * gradient will be taken). out_sig (optional, [N*M,32], ABI 7): sigmoid(o[1+k]) for the channels of sigmoid_mask, 0 for the others;
+ * p3d_decoder_mlp_bwd forms the sigmoid derivative from it (pass NULL when no gradient will be taken or the mask is 0). rgb, sigma
+ * and the pre-activations do not depend on whether out_pre / out_sig are given. One launch instead of mean + addmm + softplus +
+ * addmm + slices + sigmoid + cat. */
 int p3d_decoder_mlp_fwd(const float* feats, int64_t N, int64_t M, const float* w1, const float* b1, const float* w2,
                         const float* b2, uint32_t sigmoid_mask, float* out_rgb, float* out_sigma, float* out_pre,
-                        p3d_stream_t stream);
+                        float* out_sig, p3d_stream_t stream);
 
 /* First-order backward of p3d_decoder_mlp_fwd (what autograd derives from the module's forward): g_rgb [N*M,32] / g_sigma [N*M]
  * (either may be NULL = zeros) -> g_feats [N,3,M,32] and g_params [4257] = dL/dw1 [64,32] | dL/db1 [64] | dL/dw2 [33,64] |
- * dL/db2 [33]. pre / out_rgb: the forward's out_pre and out_rgb (nothing of the forward GEMMs is recomputed; the sigmoid
- * derivative follows from the output). Parameter gradients are accumulated per CTA and added in a fixed order (deterministic).
+ * dL/db2 [33]. pre / sig: the forward's out_pre and out_sig (nothing of the forward GEMMs is recomputed; sig may be NULL when
+ * sigmoid_mask is 0). The sigmoid derivative is g * 1.002 * (1 - s) * s in autograd's order (ABI 7; before, it was recovered from
+ * the forward's rgb output, which loses s near 0 and 1). Parameter gradients are accumulated per CTA and added in a fixed order (deterministic).
  * workspace: fp32 scratch of at least p3d_decoder_mlp_bwd_workspace_floats() elements. */
 int p3d_decoder_mlp_bwd_workspace_floats(void);
-int p3d_decoder_mlp_bwd(const float* feats, const float* pre, const float* out_rgb, int64_t N, int64_t M, const float* w1, const float* b1, const float* w2,
+int p3d_decoder_mlp_bwd(const float* feats, const float* pre, const float* sig, int64_t N, int64_t M, const float* w1, const float* b1, const float* w2,
                         const float* b2, uint32_t sigmoid_mask, const float* g_rgb, const float* g_sigma, float* g_feats,
                         float* g_params, float* workspace, int64_t workspace_floats, p3d_stream_t stream);
 

@@ -10,7 +10,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libp3d.so')
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 _lib = None
 
@@ -114,7 +114,7 @@ _SIGNATURES = {
                                  ctypes.POINTER(c_int32), ctypes.POINTER(c_int32), c_int, c_int, c_int, c_int, c_float,
                                  c_int, c_float, c_float, c_float, c_int64, c_void_p]),
     'p3d_decoder_mlp_fwd': (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
-                                    c_void_p, c_void_p]),
+                                    c_void_p, c_void_p, c_void_p]),
     'p3d_decoder_mlp_bwd_workspace_floats': (c_int, []),
     'p3d_decoder_mlp_bwd': (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),

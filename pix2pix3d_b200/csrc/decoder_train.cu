@@ -13,7 +13,8 @@
 // fp32 CUDA-core arithmetic with the exact library exp / log1p (the op must agree with torch's to ~1e-6: its results train the
 // network). Work per point: 4.2 kFMA forward, 8.3 kFMA backward (the forward saves the hidden pre-activations, so the backward
 // recomputes neither GEMM). Bytes per point: forward 384 in + 132 out (+ 256 for the saved pre-activations when a gradient can
-// follow); backward 384 (features) + 256 (pre-activations) + 128 (the op's rgb output: sigmoid') + 132 (upstream gradients) in,
+// follow, + 128 for the saved sigmoid values when a gradient can follow and a channel is sigmoid-masked); backward 384 (features)
+// + 256 (pre-activations) + 128 (the saved sigmoid values) + 132 (upstream gradients) in,
 // 384 out. Both kernels are bound by fp32 FMA issue (weights are broadcast from shared memory), not by memory.
 #include "decoder_common.cuh"
 
@@ -23,7 +24,7 @@ __global__ void __launch_bounds__(128) decoder_mlp_fwd_kernel(const float* __res
                                                                const float* __restrict__ w1, const float* __restrict__ b1,
                                                                const float* __restrict__ w2, const float* __restrict__ b2,
                                                                uint32_t mask, float* __restrict__ out_rgb, float* __restrict__ out_sigma,
-                                                               float* __restrict__ out_pre) {
+                                                               float* __restrict__ out_pre, float* __restrict__ out_sig) {
     __shared__ __align__(16) DecSmemW s;
     dec_load_weights(s, w1, b1, w2, b2);
     __syncthreads();
@@ -48,21 +49,27 @@ __global__ void __launch_bounds__(128) decoder_mlp_fwd_kernel(const float* __res
         float4* dst = reinterpret_cast<float4*>(out_rgb + pt * 32);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
-            float r[4];
+            float r[4], sg[4];
 #pragma unroll
             for (int t = 0; t < 4; ++t) {
                 const int k = 4 * q + t;
                 const float v = o[1 + k];
-                r[t] = ((mask >> k) & 1u) ? (1.f / (1.f + expf(-v))) * 1.002f - 0.001f : v;
+                const bool on = (mask >> k) & 1u;
+                sg[t] = on ? 1.f / (1.f + expf(-v)) : 0.f;
+                r[t] = on ? sg[t] * 1.002f - 0.001f : v;
             }
             dst[q] = make_float4(r[0], r[1], r[2], r[3]);
+            if (out_sig) reinterpret_cast<float4*>(out_sig + pt * 32)[q] = make_float4(sg[0], sg[1], sg[2], sg[3]);
         }
     }
 }
 
 // ---------------------------------------------------------------------------------------------
-// backward: tiles of 64 points per CTA of 128 threads. The forward saved the hidden pre-activations a1 [points, 64]; together with
-// the op's own output (sigmoid'(o) = s (1 - s) with s = (rgb + 0.001) / 1.002) nothing of the forward GEMMs is recomputed.
+// backward: tiles of 64 points per CTA of 128 threads. The forward saved the hidden pre-activations a1 [points, 64] and the sigmoid
+// values s of the masked channels, so nothing of the forward GEMMs is recomputed. sigmoid'(o) is formed from s as autograd forms it
+// (grad * 1.002 * (1 - s) * s): recovering s from the output y = 1.002 s - 0.001 instead loses it near 0 and 1, where the inverted
+// affine's rounding error is as large as 1 - s or s itself (for logits beyond about +-15 the derivative came out with the wrong sign
+// or several times too large).
 // Phase A: a lane PAIR owns a point and splits the 64 hidden units: h = softplus(a1), dL/dh = W2^T dL/do, dL/da1 = dL/dh * sigmoid(a1),
 // partial dL/dx = W1^T dL/da1 (exchanged with shuffles). Phase B: the CTA turns the tile's rows of (h, dL/da1, dL/do, x) kept in
 // shared memory into parameter-gradient contributions (thread = half a row of dW2 and dW1, looping over the tile's points);
@@ -85,7 +92,7 @@ struct DecSmemBwd {
 };
 
 __global__ void __launch_bounds__(128, kBwdCtasPerSm) decoder_mlp_bwd_kernel(const float* __restrict__ feats, const float* __restrict__ pre,
-                                                               const float* __restrict__ out_rgb, int64_t N, int64_t M,
+                                                               const float* __restrict__ sig, int64_t N, int64_t M,
                                                                const float* __restrict__ w1, const float* __restrict__ b1,
                                                                const float* __restrict__ w2, const float* __restrict__ b2, uint32_t mask,
                                                                const float* __restrict__ g_rgb, const float* __restrict__ g_sigma,
@@ -130,18 +137,15 @@ __global__ void __launch_bounds__(128, kBwdCtasPerSm) decoder_mlp_bwd_kernel(con
         o[0] = (valid && g_sigma) ? __ldg(g_sigma + pt) : 0.f;
 #pragma unroll
         for (int qq = 0; qq < 8; ++qq) {
-            float4 g = make_float4(0.f, 0.f, 0.f, 0.f), yv = g;
+            float4 g = make_float4(0.f, 0.f, 0.f, 0.f), sv = g;
             if (valid && g_rgb) g = __ldg(reinterpret_cast<const float4*>(g_rgb + pt * 32) + qq);
-            if (valid && mask) yv = __ldg(reinterpret_cast<const float4*>(out_rgb + pt * 32) + qq);
-            const float gv[4] = {g.x, g.y, g.z, g.w}, yy[4] = {yv.x, yv.y, yv.z, yv.w};
+            if (valid && mask) sv = __ldg(reinterpret_cast<const float4*>(sig + pt * 32) + qq);
+            const float gv[4] = {g.x, g.y, g.z, g.w}, ss[4] = {sv.x, sv.y, sv.z, sv.w};
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 const int k = 4 * qq + u;
                 float d = gv[u];
-                if ((mask >> k) & 1u) {
-                    const float sg = (yy[u] + 0.001f) * (1.f / 1.002f);      // y = 1.002 s - 0.001
-                    d *= 1.002f * (sg * (1.f - sg));
-                }
+                if ((mask >> k) & 1u) d = __fmul_rn(__fmul_rn(__fmul_rn(d, 1.002f), 1.f - ss[u]), ss[u]);   // ATen's order
                 o[1 + k] = d;
             }
         }
@@ -252,33 +256,34 @@ using namespace p3d;
 
 extern "C" int p3d_decoder_mlp_fwd(const float* feats, int64_t N, int64_t M, const float* w1, const float* b1, const float* w2,
                                    const float* b2, uint32_t sigmoid_mask, float* out_rgb, float* out_sigma, float* out_pre,
-                                   p3d_stream_t stream) {
+                                   float* out_sig, p3d_stream_t stream) {
     if (!feats || !w1 || !b1 || !w2 || !b2 || !out_rgb || !out_sigma || N <= 0 || M <= 0) return P3D_BAD_ARG;
-    if (((((uintptr_t)feats) | ((uintptr_t)out_rgb) | ((uintptr_t)out_pre)) & 15) != 0) return P3D_BAD_ARG;
+    if (((((uintptr_t)feats) | ((uintptr_t)out_rgb) | ((uintptr_t)out_pre) | ((uintptr_t)out_sig)) & 15) != 0) return P3D_BAD_ARG;
     const int64_t P = N * M;
     int64_t blocks = (P + 127) / 128;
     const int64_t cap = (int64_t)sm_count() * 8;
     if (blocks > cap) blocks = cap;
     decoder_mlp_fwd_kernel<<<(unsigned)blocks, 128, 0, (cudaStream_t)stream>>>(feats, N, M, w1, b1, w2, b2, sigmoid_mask, out_rgb, out_sigma,
-                                                                                  out_pre);
+                                                                                  out_pre, out_sig);
     P3D_LAUNCH_CHECK();
     return P3D_OK;
 }
 
 extern "C" int p3d_decoder_mlp_bwd_workspace_floats(void) { return sm_count() * kBwdCtasPerSm * kDecParams; }
 
-extern "C" int p3d_decoder_mlp_bwd(const float* feats, const float* pre, const float* out_rgb, int64_t N, int64_t M, const float* w1, const float* b1, const float* w2,
+extern "C" int p3d_decoder_mlp_bwd(const float* feats, const float* pre, const float* sig, int64_t N, int64_t M, const float* w1, const float* b1, const float* w2,
                                    const float* b2, uint32_t sigmoid_mask, const float* g_rgb, const float* g_sigma, float* g_feats,
                                    float* g_params, float* workspace, int64_t workspace_floats, p3d_stream_t stream) {
-    if (!feats || !pre || !out_rgb || !w1 || !b1 || !w2 || !b2 || !g_feats || !g_params || !workspace || N <= 0 || M <= 0) return P3D_BAD_ARG;
-    if (((((uintptr_t)feats) | ((uintptr_t)pre) | ((uintptr_t)out_rgb) | ((uintptr_t)g_feats) | ((uintptr_t)g_rgb)) & 15) != 0) return P3D_BAD_ARG;
+    if (!feats || !pre || (sigmoid_mask && !sig) || !w1 || !b1 || !w2 || !b2 || !g_feats || !g_params || !workspace || N <= 0 || M <= 0)
+        return P3D_BAD_ARG;
+    if (((((uintptr_t)feats) | ((uintptr_t)pre) | ((uintptr_t)sig) | ((uintptr_t)g_feats) | ((uintptr_t)g_rgb)) & 15) != 0) return P3D_BAD_ARG;
     const int64_t P = N * M, n_tiles = (P + kBwdTile - 1) / kBwdTile;
     int64_t ctas = (int64_t)sm_count() * kBwdCtasPerSm;
     if (ctas > n_tiles) ctas = n_tiles;
     if (workspace_floats < ctas * kDecParams) return P3D_BAD_ARG;
     const size_t smem = sizeof(DecSmemBwd);
     P3D_CUDA_TRY(cudaFuncSetAttribute(decoder_mlp_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    decoder_mlp_bwd_kernel<<<(unsigned)ctas, 128, smem, (cudaStream_t)stream>>>(feats, pre, out_rgb, N, M, w1, b1, w2, b2, sigmoid_mask, g_rgb,
+    decoder_mlp_bwd_kernel<<<(unsigned)ctas, 128, smem, (cudaStream_t)stream>>>(feats, pre, sig, N, M, w1, b1, w2, b2, sigmoid_mask, g_rgb,
                                                                                g_sigma, g_feats, workspace);
     P3D_LAUNCH_CHECK();
     decoder_mlp_reduce_kernel<<<ceil_div(kDecParams, 256), 256, 0, (cudaStream_t)stream>>>(workspace, (int)ctas, g_params);

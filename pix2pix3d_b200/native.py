@@ -152,7 +152,7 @@ def ray_limits_box(rays_o, rays_d, box_side_length):
 def _out_view(buf, shape, dtype, dev):
     """The leading elements of a caller's flat output buffer, viewed as `shape`."""
     n = int(np.prod(shape))
-    assert buf.dtype == dtype and buf.device == dev and buf.is_contiguous() and buf.numel() >= n, 'render_fwd out= buffer'
+    assert buf.dtype == dtype and buf.device == dev and buf.is_contiguous() and buf.numel() >= n, 'out= buffer'
     return buf.reshape(-1)[:n].view(shape)
 
 
@@ -369,12 +369,18 @@ def run_model(planes_nhwc, dec, coords, box_warp, impl=None, sigma_only=False):
     return rgb, sigma
 
 
-def sample_from_planes(planes_nhwc, coords, box_warp):
-    """coords [B,M,3] -> features [B,3,M,32] (reference layout of sample_from_planes)."""
+def _alloc(out, shape, dev, dtype=torch.float32):
+    """A fresh tensor, or the leading elements of the caller's flat buffer `out` (tests prefill longer buffers and check that a
+    launch writes nothing past its own elements)."""
+    return torch.empty(*shape, device=dev, dtype=dtype) if out is None else _out_view(out, shape, dtype, dev)
+
+
+def sample_from_planes(planes_nhwc, coords, box_warp, out=None):
+    """coords [B,M,3] -> features [B,3,M,32] (reference layout of sample_from_planes). `out`: optional buffer (see _alloc)."""
     B, _, H, W, _ = planes_nhwc.shape
     c = _f32c(coords)
     M = c.shape[1]
-    out = torch.empty(B, 3, M, 32, device=planes_nhwc.device, dtype=torch.float32)
+    out = _alloc(out, (B, 3, M, 32), planes_nhwc.device)
     with torch.cuda.device(planes_nhwc.device):
         st = _lib.lib().p3d_sample_from_planes(_lib.ptr(planes_nhwc), _lib.ptr(c), B, M, H, W, 2.0 / float(box_warp),
                                                _lib.ptr(out), _lib.stream_ptr())
@@ -383,14 +389,16 @@ def sample_from_planes(planes_nhwc, coords, box_warp):
     return out
 
 
-def ray_march(colors, densities, depths, white_back=False):
-    """MipRayMarcher2.run_forward on [B,R,S,C] / [B,R,S,1] / [B,R,S,1] tensors."""
+def ray_march(colors, densities, depths, white_back=False, out=None):
+    """MipRayMarcher2.run_forward on [B,R,S,C] / [B,R,S,1] / [B,R,S,1] tensors. `out`: optional dict of buffers keyed rgb,
+    depth, weights (see _alloc)."""
     B, R, S, Cc = colors.shape
     col, den, dep = _f32c(colors), _f32c(densities), _f32c(depths)
     dev = col.device
-    rgb = torch.empty(B, R, Cc, device=dev, dtype=torch.float32)
-    depth = torch.empty(B, R, 1, device=dev, dtype=torch.float32)
-    weights = torch.empty(B, R, S - 1, 1, device=dev, dtype=torch.float32)
+    out = out or {}
+    rgb = _alloc(out.get('rgb'), (B, R, Cc), dev)
+    depth = _alloc(out.get('depth'), (B, R, 1), dev)
+    weights = _alloc(out.get('weights'), (B, R, S - 1, 1), dev)
     ws = torch.empty(4, device=dev, dtype=torch.int32)
     with torch.cuda.device(dev):
         st = _lib.lib().p3d_ray_march(_lib.ptr(col), _lib.ptr(den), _lib.ptr(dep), B * R, S, Cc, 1 if white_back else 0,
@@ -400,12 +408,12 @@ def ray_march(colors, densities, depths, white_back=False):
     return rgb, depth, weights
 
 
-def sample_from_planes_bwd(grad_features, coords, box_warp, H, W):
-    """grad_features [B,3,M,32] -> gradient w.r.t. channels-last planes [B,3,H,W,32]."""
+def sample_from_planes_bwd(grad_features, coords, box_warp, H, W, out=None):
+    """grad_features [B,3,M,32] -> gradient w.r.t. channels-last planes [B,3,H,W,32]. `out`: optional buffer (see _alloc)."""
     g = _f32c(grad_features)
     c = _f32c(coords)
     B, _, M, _ = g.shape
-    out = torch.empty(B, 3, H, W, 32, device=g.device, dtype=torch.float32)
+    out = _alloc(out, (B, 3, H, W, 32), g.device)
     with torch.cuda.device(g.device):
         st = _lib.lib().p3d_sample_from_planes_bwd(_lib.ptr(g), _lib.ptr(c), B, M, H, W, 2.0 / float(box_warp), _lib.ptr(out),
                                                    _lib.stream_ptr())
@@ -414,16 +422,18 @@ def sample_from_planes_bwd(grad_features, coords, box_warp, H, W):
     return out
 
 
-def ray_march_bwd(colors, densities, depths, g_rgb, g_depth, g_weights, depth_range, white_back=False):
-    """Gradients of MipRayMarcher2.run_forward w.r.t. colors [B,R,S,C] and densities [B,R,S,1]."""
+def ray_march_bwd(colors, densities, depths, g_rgb, g_depth, g_weights, depth_range, white_back=False, out=None):
+    """Gradients of MipRayMarcher2.run_forward w.r.t. colors [B,R,S,C] and densities [B,R,S,1]. `out`: optional dict of
+    buffers keyed colors, densities (see _alloc)."""
     B, R, S, Cc = colors.shape
     col, den, dep = _f32c(colors), _f32c(densities), _f32c(depths)
     grgb = _f32c(g_rgb)
     gdep = None if g_depth is None else _f32c(g_depth)
     gw = None if g_weights is None else _f32c(g_weights)
     rng = None if depth_range is None else _f32c(depth_range)
-    g_col = torch.empty_like(col)
-    g_den = torch.empty_like(den)
+    out = out or {}
+    g_col = _alloc(out.get('colors'), tuple(col.shape), col.device)
+    g_den = _alloc(out.get('densities'), tuple(den.shape), col.device)
     with torch.cuda.device(col.device):
         st = _lib.lib().p3d_ray_march_bwd(_lib.ptr(col), _lib.ptr(den), _lib.ptr(dep), _lib.ptr(grgb), _lib.ptr(gdep),
                                           _lib.ptr(gw), _lib.ptr(rng), B * R, S, Cc, 1 if white_back else 0, _lib.ptr(g_col),
@@ -433,13 +443,15 @@ def ray_march_bwd(colors, densities, depths, g_rgb, g_depth, g_weights, depth_ra
     return g_col, g_den
 
 
-def sample_importance(z_vals, weights, u, return_inds=False):
-    """z_vals [N,S], weights [N,S-1], u [N,Sf] -> samples [N,Sf] (and searchsorted indices)."""
+def sample_importance(z_vals, weights, u, return_inds=False, out=None):
+    """z_vals [N,S], weights [N,S-1], u [N,Sf] -> samples [N,Sf] (and searchsorted indices). `out`: optional dict of buffers
+    keyed samples, inds (see _alloc)."""
     z, w, uu = _f32c(z_vals), _f32c(weights), _f32c(u)
     N, S = z.shape
     Sf = uu.shape[1]
-    out = torch.empty(N, Sf, device=z.device, dtype=torch.float32)
-    inds = torch.empty(N, Sf, device=z.device, dtype=torch.int32) if return_inds else None
+    bufs = out or {}
+    out = _alloc(bufs.get('samples'), (N, Sf), z.device)
+    inds = _alloc(bufs.get('inds'), (N, Sf), z.device, torch.int32) if return_inds else None
     with torch.cuda.device(z.device):
         st = _lib.lib().p3d_sample_importance(_lib.ptr(z), _lib.ptr(w), _lib.ptr(uu), N, S, Sf, _lib.ptr(out),
                                               _lib.ptr(inds), _lib.stream_ptr())
@@ -454,6 +466,49 @@ def sample_importance(z_vals, weights, u, return_inds=False):
 DECODER_PARAM_FLOATS = 64 * 32 + 64 + 33 * 64 + 33
 
 
+def decoder_mlp_fwd(feats, w1, b1, w2, b2, mask, want_saved=False, out=None):
+    """One p3d_decoder_mlp_fwd launch: feats [N,3,M,32] and EFFECTIVE parameters -> dict(rgb [N,M,32], sigma [N,M,1]); with
+    `want_saved` also pre [N*M,64] (hidden pre-activations) and, when `mask` is not 0, sig [N*M,32] (sigmoid values of the masked
+    channels), which decoder_mlp_bwd consumes. `out`: optional dict of buffers under the same keys (see _alloc)."""
+    f, w1c, b1c, w2c, b2c = (_f32c(t.detach()) for t in (feats, w1, b1, w2, b2))
+    n, _, m, _ = f.shape
+    out = out or {}
+    r = dict(rgb=_alloc(out.get('rgb'), (n, m, 32), f.device), sigma=_alloc(out.get('sigma'), (n, m, 1), f.device))
+    if want_saved:
+        r['pre'] = _alloc(out.get('pre'), (n * m, 64), f.device)
+        if mask:
+            r['sig'] = _alloc(out.get('sig'), (n * m, 32), f.device)
+    with torch.cuda.device(f.device):
+        st = _lib.lib().p3d_decoder_mlp_fwd(_lib.ptr(f), n, m, _lib.ptr(w1c), _lib.ptr(b1c), _lib.ptr(w2c), _lib.ptr(b2c), int(mask),
+                                            _lib.ptr(r['rgb']), _lib.ptr(r['sigma']), _lib.ptr(r.get('pre')), _lib.ptr(r.get('sig')),
+                                            _lib.stream_ptr())
+    _lib.check(st, 'p3d_decoder_mlp_fwd')
+    _lib.bump()
+    return r
+
+
+def decoder_mlp_bwd(feats, w1, b1, w2, b2, mask, pre, sig, g_rgb, g_sigma, out=None):
+    """One p3d_decoder_mlp_bwd launch: the forward's inputs, its saved pre / sig (decoder_mlp_fwd with want_saved) and the upstream
+    gradients g_rgb [N,M,32] / g_sigma [N,M,1] (either may be None) -> dict(feats = dL/dfeats [N,3,M,32], params = dL/d(w1 | b1 |
+    w2 | b2) [4257]). `out`: optional dict of buffers keyed feats, params (see _alloc)."""
+    f, w1c, b1c, w2c, b2c = (_f32c(t.detach()) for t in (feats, w1, b1, w2, b2))
+    n, _, m, _ = f.shape
+    gr = None if g_rgb is None else _f32c(g_rgb)
+    gs = None if g_sigma is None else _f32c(g_sigma)
+    out = out or {}
+    g_feats = _alloc(out.get('feats'), tuple(f.shape), f.device)
+    g_params = _alloc(out.get('params'), (DECODER_PARAM_FLOATS,), f.device)
+    with torch.cuda.device(f.device):
+        nws = _lib.lib().p3d_decoder_mlp_bwd_workspace_floats()
+        ws = torch.empty(nws, device=f.device, dtype=torch.float32)
+        st = _lib.lib().p3d_decoder_mlp_bwd(_lib.ptr(f), _lib.ptr(pre), _lib.ptr(sig), n, m, _lib.ptr(w1c), _lib.ptr(b1c), _lib.ptr(w2c),
+                                            _lib.ptr(b2c), int(mask), _lib.ptr(gr), _lib.ptr(gs), _lib.ptr(g_feats), _lib.ptr(g_params),
+                                            _lib.ptr(ws), nws, _lib.stream_ptr())
+    _lib.check(st, 'p3d_decoder_mlp_bwd')
+    _lib.bump(2)
+    return dict(feats=g_feats, params=g_params)
+
+
 class _DecoderMLP(torch.autograd.Function):
     """feats [N,3,M,32] -> (rgb [N,M,32], sigma [N,M,1]) through mean(1) -> FC(32,64) -> softplus -> FC(64,33) [-> sigmoid], forward
     and first-order backward on libp3d. w1 / b1 / w2 / b2 are the EFFECTIVE parameters (runtime gains applied by the caller under
@@ -462,38 +517,21 @@ class _DecoderMLP(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feats, w1, b1, w2, b2, mask):
         f, w1c, b1c, w2c, b2c = (_f32c(t.detach()) for t in (feats, w1, b1, w2, b2))
-        n, _, m, _ = f.shape
-        rgb = torch.empty(n, m, 32, device=f.device, dtype=torch.float32)
-        sigma = torch.empty(n, m, 1, device=f.device, dtype=torch.float32)
-        # hidden pre-activations for the backward pass (256 bytes per point), only when a gradient can be asked for
-        pre = torch.empty(n * m, 64, device=f.device, dtype=torch.float32) if any(ctx.needs_input_grad) else None
-        with torch.cuda.device(f.device):
-            st = _lib.lib().p3d_decoder_mlp_fwd(_lib.ptr(f), n, m, _lib.ptr(w1c), _lib.ptr(b1c), _lib.ptr(w2c), _lib.ptr(b2c), int(mask),
-                                                _lib.ptr(rgb), _lib.ptr(sigma), _lib.ptr(pre), _lib.stream_ptr())
-        _lib.check(st, 'p3d_decoder_mlp_fwd')
-        _lib.bump()
-        if pre is not None:
-            ctx.save_for_backward(f, w1c, b1c, w2c, b2c, pre, rgb)
+        # the hidden pre-activations (256 bytes per point) and the sigmoid values (128) for the backward pass, only when a
+        # gradient can be asked for
+        grad = any(ctx.needs_input_grad)
+        r = decoder_mlp_fwd(f, w1c, b1c, w2c, b2c, int(mask), want_saved=grad)
+        if grad:
+            ctx.save_for_backward(f, w1c, b1c, w2c, b2c, r['pre'], r.get('sig'))
         ctx.mask = int(mask)
-        return rgb, sigma
+        return r['rgb'], r['sigma']
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, g_rgb, g_sigma):
-        f, w1, b1, w2, b2, pre, rgb = ctx.saved_tensors
-        n, _, m, _ = f.shape
-        gr = None if g_rgb is None else _f32c(g_rgb)
-        gs = None if g_sigma is None else _f32c(g_sigma)
-        g_feats = torch.empty_like(f)
-        g_params = torch.empty(DECODER_PARAM_FLOATS, device=f.device, dtype=torch.float32)
-        with torch.cuda.device(f.device):
-            nws = _lib.lib().p3d_decoder_mlp_bwd_workspace_floats()
-            ws = torch.empty(nws, device=f.device, dtype=torch.float32)
-            st = _lib.lib().p3d_decoder_mlp_bwd(_lib.ptr(f), _lib.ptr(pre), _lib.ptr(rgb), n, m, _lib.ptr(w1), _lib.ptr(b1), _lib.ptr(w2), _lib.ptr(b2), ctx.mask,
-                                                _lib.ptr(gr), _lib.ptr(gs), _lib.ptr(g_feats), _lib.ptr(g_params), _lib.ptr(ws), nws,
-                                                _lib.stream_ptr())
-        _lib.check(st, 'p3d_decoder_mlp_bwd')
-        _lib.bump(2)
+        f, w1, b1, w2, b2, pre, sig = ctx.saved_tensors
+        g = decoder_mlp_bwd(f, w1, b1, w2, b2, ctx.mask, pre, sig, g_rgb, g_sigma)
+        g_feats, g_params = g['feats'], g['params']
         gw1, gb1, gw2, gb2 = torch.split(g_params, [64 * 32, 64, 33 * 64, 33])
         return g_feats, gw1.view(64, 32), gb1, gw2.view(33, 64), gb2, None
 
