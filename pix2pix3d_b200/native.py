@@ -281,12 +281,13 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
 
 
 def render_bwd(planes_nhwc, params, sigma_net, masks, ray_origins, ray_dirs, depths_sorted, Sc, Sf, box_warp, g_feat, g_depth=None,
-               g_wsum=None, depth_range=None, white_back=False, want_planes=True, want_params=True):
+               g_wsum=None, depth_range=None, white_back=False, want_planes=True, want_params=True, out=None):
     """First-order backward of render_fwd (p3d_render_bwd): recomputes every ray from the planes [B,3,H,W,32], its sorted
     depths [B,R,Sc+Sf] (render_fwd's out['depths_sorted']) and the decoder's EFFECTIVE parameters `params` (per net
     (w1, b1, w2, b2) with the gains applied, as _effective_fc forms them). g_feat [B,R,C]; g_depth / g_wsum [B,R(,1)] or None;
     depth_range: device [2] = (min, max) of all depths, needed with g_depth. Returns (dL/dplanes [B,3,H,W,32] or None,
-    dL/dparams [n_nets,4257] = w1 | b1 | w2 | b2 per net, or None)."""
+    dL/dparams [n_nets,4257] = w1 | b1 | w2 | b2 per net, or None). `out`: optional dict of buffers keyed planes, params
+    (see _alloc) and workspace (the per-CTA parameter partials; its whole length is passed to the launch)."""
     B, _, H, W, C = planes_nhwc.shape
     assert C == 32 and planes_nhwc.dtype == torch.float32
     p = _f32c(planes_nhwc)
@@ -315,14 +316,18 @@ def render_bwd(planes_nhwc, params, sigma_net, masks, ray_origins, ray_dirs, dep
             keep.append(t)
             setattr(a, name, t.data_ptr())
     dev = p.device
-    g_planes = torch.empty(B, 3, H, W, 32, device=dev, dtype=torch.float32) if want_planes else None
+    out = out or {}
+    g_planes = _alloc(out.get('planes'), (B, 3, H, W, 32), dev) if want_planes else None
     g_params = None
     with torch.cuda.device(dev):
         if want_params:
-            g_params = torch.empty(n_nets, DECODER_PARAM_FLOATS, device=dev, dtype=torch.float32)
-            nws = _lib.lib().p3d_render_bwd_workspace_floats(n_nets)
-            ws = torch.empty(nws, device=dev, dtype=torch.float32)
-            a.g_params, a.workspace, a.workspace_floats = g_params.data_ptr(), ws.data_ptr(), nws
+            g_params = _alloc(out.get('params'), (n_nets, DECODER_PARAM_FLOATS), dev)
+            ws = out.get('workspace')
+            if ws is None:
+                ws = torch.empty(_lib.lib().p3d_render_bwd_workspace_floats(n_nets), device=dev, dtype=torch.float32)
+            else:
+                assert ws.dtype == torch.float32 and ws.device == dev and ws.is_contiguous(), 'out= buffer'
+            a.g_params, a.workspace, a.workspace_floats = g_params.data_ptr(), ws.data_ptr(), ws.numel()
         if want_planes:
             a.g_planes_nhwc = g_planes.data_ptr()
         st = _lib.lib().p3d_render_bwd(ctypes.byref(a), _lib.stream_ptr())
