@@ -385,6 +385,39 @@ int p3d_conv_gemm(const p3d_conv_args_t* args, p3d_stream_t stream);
  * Results are identical to n_phases separate p3d_conv_gemm calls. */
 int p3d_conv_gemm_phases(const p3d_conv_args_t* phases, int n_phases, p3d_stream_t stream);
 
+/* Weight gradient of the fp32 training convolutions (the weight-gradient op of conv2d_gradfix.py:150-170) as one tensor-core
+ * GEMM whose reduction runs over pixels:
+ *   dw[m][n][t] = sum_{b, g} P[b][m][g] * Q[b][tap_phase[t]][n][g + tap_off[t]] / (*p_scale) / (*q_scale)
+ * P and Q are hi/lo fp16 planes (three passes, hi*hi + hi*lo + lo*hi) written by p3d_wgrad_operand: flattened grids of Lp
+ * (P) and Lq (Q) pixels per (image, channel) row, both multiples of 8; g runs over [0, Lp) and Q reads past Lq are zero.
+ * tap_off[t] must be a non-negative multiple of 8 (TMA box starts are 16-byte aligned): a tap's horizontal shift is a
+ * phase of Q, its vertical shift a multiple of the grid width. The reduction is split over `splits` CTAs per output tile
+ * (1 <= splits <= B * ceil(Lp / 64)); the partial tiles go to `scratch` (at least splits * n_taps * Mp * Np floats,
+ * Mp = 128 * ceil(M / 128), Np = BN * ceil(N / BN), BN = 128 / 64 / 32 for N > 64 / > 32 / else) and a second kernel sums
+ * them in a fixed order, so dw is bit-reproducible. With P = dY, Q = X: a stride-1 convolution's dw [Cout][Cin][k][k] or a
+ * stride-2 'valid' 3x3 one's; with P = X, Q = dY: a stride-2 transposed 3x3 one's (torch's [Cin][Cout][3][3]). */
+typedef struct {
+    const void* p;            /* [2][B][M][Lp] fp16 */
+    const void* q;            /* [2][B][q_phases][N][Lq] fp16 */
+    int32_t B, M, N, Lp, Lq, q_phases, n_taps;
+    int32_t tap_phase[9], tap_off[9];
+    int32_t splits;
+    float* scratch;
+    int64_t scratch_bytes;
+    const float* p_scale;     /* device scalars: the powers of two the operands were multiplied by */
+    const float* q_scale;
+    float* dw;                /* [M][N][n_taps] fp32 */
+} p3d_wgrad_args_t;
+int p3d_conv_wgrad(const p3d_wgrad_args_t* args, p3d_stream_t stream);
+
+/* Operand of p3d_conv_wgrad: x fp32 NCHW [B][C][H][W] -> out fp16 [2][B][n_phases][C][Hg * Wp] = hi, lo of x * (*scale)
+ * (scale NULL: 1), Wp % 8 == 0. Grid position (gy, gx) of phase ph holds
+ *   stride 1 (n_phases odd): x[gy - oy][gx + ph - (n_phases - 1) / 2]
+ *   stride 2 (n_phases = 6): x[2 (gy - oy) + ph / 3][2 (gx + ((ph % 3) >> 1)) + ((ph % 3) & 1)]
+ * and zero where that lies outside the image. */
+int p3d_wgrad_operand(const float* x, int B, int C, int H, int W, int stride, int n_phases, int Hg, int Wp, int oy,
+                      const float* scale, void* out, p3d_stream_t stream);
+
 /* Per-sample modulated (and optionally demodulated) weights, modulated_conv2d lines :58-67:
  *   w'[b,o,i,k] = weight[o,i,k] * styles[b,i];  d[b,o] = rsqrt(sum_{i,k} w'^2 + 1e-8);  out = w' * d * scale
  * written K-major [planes][B][Cout_padded][kh*kw][Cin_padded] as fp16 (planes = 2: hi/lo split). Rows >= Cout and

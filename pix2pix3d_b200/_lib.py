@@ -10,7 +10,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libp3d.so')
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 _lib = None
 
@@ -123,6 +123,9 @@ _SIGNATURES = {
     'p3d_fma': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'p3d_conv_gemm': (c_int, [c_void_p, c_void_p]),
     'p3d_conv_gemm_phases': (c_int, [c_void_p, c_int, c_void_p]),
+    'p3d_conv_wgrad': (c_int, [c_void_p, c_void_p]),
+    'p3d_wgrad_operand': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                  c_void_p]),
     'p3d_prepare_weights': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'p3d_modulate_weights_t': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
                                        c_float, c_int, c_void_p, c_void_p]),

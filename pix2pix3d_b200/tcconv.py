@@ -226,8 +226,9 @@ def _conv_args(x, w, cout, taps, grid_hw, out, out_lo=None, out_mode=0, out_map=
     return a
 
 
-def _launch(device, call, name, flops, split):
-    """Run one libp3d convolution launch; with native.kernel_events set, bracket it with CUDA events (bench.py's tensor roofline)."""
+def _launch(device, call, name, flops, split, tag='conv_gemm'):
+    """Run one libp3d convolution launch; with native.kernel_events set, bracket it with CUDA events (bench.py's tensor roofline
+    counts the 'conv_gemm' ones)."""
     from . import native
     ev = None
     if native.kernel_events is not None:
@@ -239,7 +240,7 @@ def _launch(device, call, name, flops, split):
         ev[1].record()
         # algorithmic FLOPs of the convolution this launch implements (one pass); the fp32 layers execute 3x that on the
         # tensor pipe (hi*hi + hi*lo + lo*hi)
-        native.kernel_events.append(('conv_gemm', ev[0], ev[1], flops, flops * (3 if split else 1)))
+        native.kernel_events.append((tag, ev[0], ev[1], flops, flops * (3 if split else 1)))
     _lib.check(st, name)
     _lib.bump()
 
@@ -376,3 +377,123 @@ def upsample2x_nhwc(x, f, out=None):
     _lib.check(st, 'p3d_upsample2x_nhwc')
     _lib.bump()
     return y
+
+
+# ----------------------------------------------------------------------------------------------
+# weight gradients (p3d_conv_wgrad)
+# ----------------------------------------------------------------------------------------------
+class WgradArgs(ctypes.Structure):  # p3d_wgrad_args_t
+    _fields_ = [
+        ('p', ctypes.c_void_p), ('q', ctypes.c_void_p),
+        ('B', ctypes.c_int32), ('M', ctypes.c_int32), ('N', ctypes.c_int32), ('Lp', ctypes.c_int32), ('Lq', ctypes.c_int32),
+        ('q_phases', ctypes.c_int32), ('n_taps', ctypes.c_int32),
+        ('tap_phase', ctypes.c_int32 * 9), ('tap_off', ctypes.c_int32 * 9),
+        ('splits', ctypes.c_int32),
+        ('scratch', ctypes.c_void_p), ('scratch_bytes', ctypes.c_int64),
+        ('p_scale', ctypes.c_void_p), ('q_scale', ctypes.c_void_p), ('dw', ctypes.c_void_p),
+    ]
+
+
+WGRAD_BM, WGRAD_BK = 128, 64       # P channels per tile, pixels per k-step (conv_wgrad.cu)
+WGRAD_MAX_SPLITS = 64
+
+
+def wgrad_plan(b, m, n, hw, k, stride, sms, splits=None):
+    """Geometry of dW[m, n, ky, kx] = sum_{b,y,x} P[b,m,y,x] Q[b,n,s*y+ky-pad, s*x+kx-pad] as p3d_conv_wgrad runs it. P is
+    [b,m,H,W] (hw = (H, W)); Q is [b,n,H,W] with pad = k // 2 at stride 1, [b,n,2H+1,2W+1] with pad = 0 at stride 2 (3x3).
+
+    Both operands live on grids of Wp-pixel rows (Wp = W rounded up to 8, so that TMA box starts stay 16-byte aligned),
+    flattened per (image, channel): P on an H x Wp grid, Q as `q_phases` copies on an Hq x Wp grid. A tap's horizontal
+    shift is baked into a Q phase and its vertical shift is a whole number of rows, `off` (p3d_wgrad_operand):
+    - stride 1: phase kx = Q shifted by kx - pad columns, with pad zero rows on top (Hq = H + 2 pad); off = ky * Wp;
+    - stride 2: phase 3 (ky & 1) + kx = Q[2 gy + (ky & 1)][2 (gx + (kx >> 1)) + (kx & 1)] (Hq = H + 1); off = (ky >> 1) * Wp.
+    P pixel (y, x) then meets the Q pixel of its tap at grid position (y, x) + off: no term crosses a grid row.
+
+    Split-K: the reduction (b * ceil(H * Wp / 64) k-steps) of each of the m_tiles x n_tiles x k^2 output tiles is cut into
+    `splits` contiguous ranges, one CTA each; unless given, `splits` minimises waves x (k-steps per CTA + 8) on `sms` SMs
+    (8 k-steps stand for a CTA's pipeline fill and partial-tile store)."""
+    h, w = hw
+    wp = pad_to(w, 8)
+    if stride == 1:
+        assert k in (1, 3)
+        pad = k // 2
+        hq, q_phases, q_top = h + 2 * pad, k, pad
+        taps = [(kx, ky * wp) for ky in range(k) for kx in range(k)]
+    else:
+        assert stride == 2 and k == 3
+        hq, q_phases, q_top = h + 1, 6, 0
+        taps = [(3 * (ky & 1) + kx, (ky >> 1) * wp) for ky in range(3) for kx in range(3)]
+    lp, lq = h * wp, hq * wp
+    bn = 128 if n > 64 else 64 if n > 32 else 32
+    m_tiles, n_tiles = -(-m // WGRAD_BM), -(-n // bn)
+    nchunks = -(-lp // WGRAD_BK)
+    total_k = b * nchunks
+    base = m_tiles * n_tiles * len(taps)
+    if splits is None:
+        best = None
+        for s in range(1, min(total_k, WGRAD_MAX_SPLITS) + 1):
+            cost = -(-base * s // sms) * (-(-total_k // s) + 8)
+            if best is None or cost < best[0]:
+                best = (cost, s)
+        splits = best[1]
+    assert 1 <= splits <= total_k
+    mp, np_ = m_tiles * WGRAD_BM, n_tiles * bn
+    return dict(stride=stride, wp=wp, hq=hq, q_top=q_top, Lp=lp, Lq=lq, q_phases=q_phases, taps=taps, bn=bn, m_tiles=m_tiles,
+                n_tiles=n_tiles, nchunks=nchunks, total_k=total_k, splits=splits,
+                ranges=[(total_k * s // splits, total_k * (s + 1) // splits) for s in range(splits)],
+                units=base * splits, scratch_floats=splits * len(taps) * mp * np_)
+
+
+def pow2_scale(t):
+    """Device scalar 2^floor(log2(1024 / amax|t|)): brings the tensor's largest magnitude to [2^10, 2^11) before an fp16
+    hi/lo split (gradients sit far below fp16's normal range, where the split has no bits left). Exact to undo; no host
+    read-back."""
+    amax = t.detach().abs().amax().clamp_min(1e-30)
+    return torch.exp2(torch.floor(torch.log2(1024.0 / amax)))
+
+
+def wgrad_operand(x, grid_h, wp, stride, phases, top, scale):
+    """x fp32 NCHW -> [2, B, phases, C, grid_h * wp] fp16 hi/lo of x * scale (p3d_wgrad_operand)."""
+    x = x.detach().contiguous()
+    assert x.is_cuda and x.dtype == torch.float32 and x.ndim == 4
+    b, c, h, w = x.shape
+    out = torch.empty(2, b, phases, c, grid_h * wp, device=x.device, dtype=torch.float16)
+    with torch.cuda.device(x.device):
+        st = _lib.lib().p3d_wgrad_operand(_lib.ptr(x), b, c, h, w, stride, phases, grid_h, wp, top, _lib.ptr(scale), _lib.ptr(out),
+                                          _lib.stream_ptr())
+    _lib.check(st, 'p3d_wgrad_operand')
+    _lib.bump()
+    return out
+
+
+def _sms(device):
+    return torch.cuda.get_device_properties(device).multi_processor_count
+
+
+def conv_wgrad(p, q, k, stride, p_scale=None, q_scale=None, splits=None):
+    """Weight gradient on the tensor cores: P [B,M,H,W], Q fp32 NCHW (see wgrad_plan) -> dW [M,N,k,k] fp32,
+    dW[m, n, ky, kx] = sum_{b,y,x} P[b,m,y,x] Q[b,n,s*y+ky-pad, s*x+kx-pad], three fp16 passes (hi*hi + hi*lo + lo*hi).
+    p_scale / q_scale: device powers of two applied before the split (pow2_scale of the operand when None)."""
+    b, m, h, w = p.shape
+    n = q.shape[1]
+    assert q.shape[0] == b
+    assert tuple(q.shape[2:]) == ((h, w) if stride == 1 else (2 * h + 1, 2 * w + 1)), (p.shape, q.shape, stride)
+    plan = wgrad_plan(b, m, n, (h, w), k, stride, _sms(p.device), splits=splits)
+    p_scale = pow2_scale(p) if p_scale is None else p_scale
+    q_scale = pow2_scale(q) if q_scale is None else q_scale
+    ph = wgrad_operand(p, h, plan['wp'], 1, 1, 0, p_scale)
+    qh = wgrad_operand(q, plan['hq'], plan['wp'], stride, plan['q_phases'], plan['q_top'], q_scale)
+    scratch = torch.empty(plan['scratch_floats'], device=p.device, dtype=torch.float32)
+    dw = torch.empty(m, n, k, k, device=p.device, dtype=torch.float32)
+    a = WgradArgs()
+    a.p, a.q = ph.data_ptr(), qh.data_ptr()
+    a.B, a.M, a.N, a.Lp, a.Lq, a.q_phases, a.n_taps = b, m, n, plan['Lp'], plan['Lq'], plan['q_phases'], len(plan['taps'])
+    for t, (phase, off) in enumerate(plan['taps']):
+        a.tap_phase[t], a.tap_off[t] = phase, off
+    a.splits = plan['splits']
+    a.scratch, a.scratch_bytes = scratch.data_ptr(), scratch.numel() * 4
+    a.p_scale, a.q_scale, a.dw = p_scale.data_ptr(), q_scale.data_ptr(), dw.data_ptr()
+    flops = 2.0 * b * h * w * m * n * k * k
+    _launch(p.device, lambda: _lib.lib().p3d_conv_wgrad(ctypes.byref(a), _lib.stream_ptr()), 'p3d_conv_wgrad', flops, True,
+            tag='conv_wgrad')
+    return dw

@@ -2,8 +2,9 @@
 
 Surface of the reference's torch_utils/ops/conv2d_gradfix.py (:23 `enabled`, :26-33 `no_weight_gradients`,
 :37-45 entry points). The forward / data-gradient / weight-gradient convolutions are ATen calls, exactly as in the reference
-(:128-129, :169) -- except inside `native_conv.first_order()` regions (the generator's training passes), where fp32 stride-1
-convolutions run forward and input gradient on libp3d's wgmma implicit GEMM (native_conv.py). The inference path does not go
+(:128-129, :169) -- except inside `native_conv.first_order()` regions (the generator's training passes), where the fp32
+stride-1, strided (down=2) and transposed (up=2) convolutions run forward, input gradient and weight gradient on libp3d's wgmma
+kernels (native_conv.py). The inference path does not go
 through this module (engine.py drives the same kernels directly).
 """
 import contextlib
@@ -37,6 +38,9 @@ def conv2d(input, weight, bias=None, stride=1, padding=0, dilation=1, groups=1):
     if native_conv.applies(input, weight, bias, _pair(stride), _pair(padding), _pair(dilation), groups):
         # fp32 training convolutions of the generator / label-map encoder: forward + input gradient on p3d_conv_gemm
         return native_conv.conv2d(input, weight)
+    if native_conv.applies_strided(input, weight, bias, _pair(stride), _pair(padding), _pair(dilation), groups):
+        # the label-map Encoder's down=2 layers: stride-2 'valid' convolution forward, phase GEMMs for the input gradient
+        return native_conv.conv2d_stride2(input, weight)
     if _use_custom(input):
         return _make_op(False, weight.shape, _pair(stride), _pair(padding), (0, 0), _pair(dilation), groups).apply(
             input, weight, bias)

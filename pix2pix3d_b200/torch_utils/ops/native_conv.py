@@ -1,17 +1,23 @@
-"""fp32 convolutions of the training path on the wgmma implicit-GEMM kernel (`p3d_conv_gemm`, three-pass fp16 split = fp32
-accuracy) instead of cuDNN's fp32 SIMT kernels (TF32 is off during training, training_loop.py:278-279, which leaves cuDNN on
-its fp32 CUDA-core kernels).
+"""fp32 convolutions of the training path on libp3d's wgmma kernels (three-pass fp16 split = fp32 accuracy) instead of cuDNN's
+fp32 SIMT kernels (TF32 is off during training, training_loop.py:278-279, which leaves cuDNN on its fp32 CUDA-core kernels).
 
 Scope: what `conv2d_gradfix.conv2d` receives from the non-fused modulated convolutions of the generator and from the label-map
 Encoder when gradients are required (`networks_stylegan2.py:68-75`, `conv2d_resample.py:134-136`): 3x3 (padding 1) and 1x1
-(padding 0), stride 1, dilation 1, groups 1, no bias, fp32 NCHW -- and what `conv2d_gradfix.conv_transpose2d` receives from the
-up=2 layers (`conv2d_resample.py:114-128`: 3x3, stride 2, padding 0 -> the (2H+1) x (2W+1) grid the FIR then filters). Forward and
-the input gradient run on libp3d (the input gradient of a stride-1 convolution is the same convolution with the kernel flipped
-and its channel axes swapped; the transposed convolution runs as its four phase GEMMs in one launch, its input gradient is a
-stride-2 'valid' convolution of the incoming gradient with the same weight tensor); the weight
-gradient stays ATen's `convolution_backward` (a tensor-core wgrad needs MN-major operand tiles: not built). First-order only: the
-node is used where no double backward can follow (inside `first_order()`, which the generator's `mapping` / `synthesis` /
-`sample_mixed` enter; the discriminators, whose R1 penalty differentiates twice, never do).
+(padding 0), stride 1, dilation 1, groups 1, no bias, fp32 NCHW; the Encoder's down=2 3x3 convolutions (`conv2d_resample.py:54-56`:
+stride 2, padding 0 on the FIR-filtered (2H+1) x (2W+1) grid); and what `conv2d_gradfix.conv_transpose2d` receives from the
+up=2 layers (`conv2d_resample.py:114-128`: 3x3, stride 2, padding 0 -> the (2H+1) x (2W+1) grid the FIR then filters).
+
+Each node runs all three of its computations on libp3d:
+- stride 1: forward and input gradient on `p3d_conv_gemm` (the input gradient is the same convolution with the kernel flipped
+  and its channel axes swapped);
+- transposed stride 2: forward as its four phase GEMMs in one launch, input gradient as a stride-2 'valid' convolution of the
+  incoming gradient with the same weight tensor;
+- strided stride 2: the reverse pair (forward = the stride-2 'valid' convolution, input gradient = the phase GEMMs);
+- the weight gradient of every node on `p3d_conv_wgrad` (tcconv.conv_wgrad): one GEMM over pixels with both operands in
+  NCHW order (pixels contiguous: the K-major tiles wgmma takes, no MN-major tiles needed), the second operand stored once per
+  horizontal tap shift so that each tap is a whole-row offset.
+First-order only: the nodes are used where no double backward can follow (inside `first_order()`, which the generator's
+`mapping` / `synthesis` / `sample_mixed` enter; the discriminators, whose R1 penalty differentiates twice, never do).
 """
 import contextlib
 
@@ -77,19 +83,17 @@ class _Conv2d(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         from . import conv2d_gradfix
+        from ... import tcconv
         x, w = ctx.saved_tensors
         dx = dw = None
+        # gradients sit far below fp16's normal range (1e-6 and less), where the hi/lo split has no bits left: bring the
+        # tensor's largest magnitude to ~2^10 with a power-of-two scale (exact), undo it on the result. The scale stays on
+        # the device (no host read-back).
+        scale = tcconv.pow2_scale(dy)
         if ctx.needs_input_grad[0]:
-            # gradients sit far below fp16's normal range (1e-6 and less), where the hi/lo split has no bits left: bring the
-            # tensor's largest magnitude to ~2^10 with a power-of-two scale (exact), undo it on the result. The scale stays on
-            # the device (no host read-back).
-            amax = dy.detach().abs().amax().clamp_min(1e-30)
-            scale = torch.exp2(torch.floor(torch.log2(1024.0 / amax)))
             dx = _conv(dy * scale, w.flip([2, 3]).transpose(0, 1).contiguous()) / scale
         if ctx.needs_input_grad[1] and not conv2d_gradfix.weight_gradients_disabled:
-            k = w.shape[2]
-            dw = torch.ops.aten.convolution_backward(dy.contiguous(), x, w, None, [1, 1], [k // 2, k // 2], [1, 1], False, [0, 0], 1,
-                                                     [False, True, False])[1]
+            dw = tcconv.conv_wgrad(dy, x, w.shape[2], 1, p_scale=scale)
         return dx, dw
 
 
@@ -158,17 +162,61 @@ class _ConvTranspose2d(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         from . import conv2d_gradfix
+        from ... import tcconv
         x, wt = ctx.saved_tensors
         dx = dw = None
+        scale = tcconv.pow2_scale(dy)          # power-of-two scaling before the fp16 split, as in _Conv2d
         if ctx.needs_input_grad[0]:
-            amax = dy.detach().abs().amax().clamp_min(1e-30)          # power-of-two scaling before the fp16 split, as in _Conv2d
-            scale = torch.exp2(torch.floor(torch.log2(1024.0 / amax)))
             dx = _conv_stride2_valid(dy * scale, wt) / scale
         if ctx.needs_input_grad[1] and not conv2d_gradfix.weight_gradients_disabled:
-            dw = torch.ops.aten.convolution_backward(dy.contiguous(), x, wt, None, [2, 2], [0, 0], [1, 1], True, [0, 0], 1,
-                                                     [False, True, False])[1]
+            dw = tcconv.conv_wgrad(x, dy, 3, 2, q_scale=scale)      # [in, out, 3, 3]: P = x, Q = the four phases of dy
         return dx, dw
 
 
 def conv_transpose2d(x, wt):
     return _ConvTranspose2d.apply(x, wt)
+
+
+# ----------------------------------------------------------------------------------------------
+# stride-2 3x3 convolution, padding 0 (the label-map Encoder's down=2 layers after their FIR)
+# ----------------------------------------------------------------------------------------------
+def applies_strided(x, w, bias, stride, padding, dilation, groups):
+    """conv2d(x [B,I,2H+1,2W+1], w [O,I,3,3], stride 2, padding 0) -> [B,O,H,W] inside a first_order() region."""
+    if not (enabled and _depth > 0 and bias is None and isinstance(x, torch.Tensor) and x.is_cuda):
+        return False
+    if x.dtype != torch.float32 or w.dtype != torch.float32 or x.ndim != 4 or tuple(w.shape[2:]) != (3, 3) or groups != 1:
+        return False
+    if tuple(stride) != (2, 2) or tuple(padding) != (0, 0) or tuple(dilation) != (1, 1) or w.shape[1] != x.shape[1]:
+        return False
+    hh, ww = x.shape[2], x.shape[3]
+    if hh % 2 == 0 or ww % 2 == 0 or (hh // 2) * (ww // 2) < min_pixels or x.shape[0] > 4096:
+        return False
+    for ch in (w.shape[0], w.shape[1]):                # channel-tile rule of the kernel, for both roles (forward / input gradient)
+        if ch > 128 and ch % 128:
+            return False
+    return torch.is_grad_enabled() and (x.requires_grad or w.requires_grad)
+
+
+class _Conv2dStride2(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w):
+        ctx.save_for_backward(x, w)
+        return _conv_stride2_valid(x, w)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        from . import conv2d_gradfix
+        from ... import tcconv
+        x, w = ctx.saved_tensors
+        dx = dw = None
+        scale = tcconv.pow2_scale(dy)
+        if ctx.needs_input_grad[0]:
+            dx = _conv_transpose(dy * scale, w) / scale          # adjoint of the stride-2 'valid' convolution
+        if ctx.needs_input_grad[1] and not conv2d_gradfix.weight_gradients_disabled:
+            dw = tcconv.conv_wgrad(dy, x, 3, 2, p_scale=scale)   # [out, in, 3, 3]: P = dy, Q = the four phases of x
+        return dx, dw
+
+
+def conv2d_stride2(x, w):
+    return _Conv2dStride2.apply(x, w)
