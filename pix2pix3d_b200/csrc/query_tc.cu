@@ -157,17 +157,9 @@ extern "C" int p3d_run_model_tc(const float* planes_nhwc, const int64_t plane_st
     P.M = (int)M; P.H = H; P.W = W; P.n_nets = n_nets; P.sigma_net = sigma_net;
     P.mask[0] = sigmoid_mask[0]; P.mask[1] = sigmoid_mask[1];
     P.coord_scale = coord_scale;
-    {
-        const int64_t psz = (int64_t)H * W * kC;
-        const bool dense = !plane_strides || !(plane_strides[0] || plane_strides[1] || plane_strides[2]);
-        const int64_t is = dense ? 3 * psz : plane_strides[0], pls = dense ? psz : plane_strides[1], pxs = dense ? kC : plane_strides[2];
-        if (is <= 0 || pls <= 0 || pxs < kC) return P3D_BAD_ARG;
-        if ((((uintptr_t)planes_nhwc) & 15) != 0 || (is & 3) || (pls & 3) || (pxs & 3)) return P3D_UNSUPPORTED;
-        if (out_rgb && (((uintptr_t)out_rgb) & 15) != 0) return P3D_UNSUPPORTED;
-        const int64_t max_off = (int64_t)(B - 1) * is + 2 * pls + ((int64_t)H * W - 1) * pxs + kC;
-        if (max_off >= ((int64_t)1 << 32)) return P3D_UNSUPPORTED;
-        P.img_stride = (uint32_t)is; P.plane_stride = (uint32_t)pls; P.pix_stride = (uint32_t)pxs;
-    }
+    if (const int st = plane_strides_status(planes_nhwc, plane_strides, B, H, W, P.img_stride, P.plane_stride, P.pix_stride))
+        return st;
+    if (out_rgb && (((uintptr_t)out_rgb) & 15) != 0) return P3D_UNSUPPORTED;
     const size_t smem = (size_t)kQSmemBytes + 1024;
     P3D_CUDA_TRY(cudaFuncSetAttribute(run_model_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     long long grid = (P.n_tiles + 2) / 3;

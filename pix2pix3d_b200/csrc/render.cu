@@ -247,8 +247,8 @@ __device__ __forceinline__ void mlp_colors8(const float* __restrict__ net, const
 // ---------------------------------------------------------------------------------------------
 struct RenderLayout {   // shared-memory carve-up (float offsets), identical on host and device
     int RT, Sc, Sf, S, Scp, Sfp, gc, gf, NGc, NGf, NT;
-    int off_dec, off_feat, off_ray, ray_stride, off_part, off_scal, total_floats;
-    int o_dC, o_sC, o_dF, o_sF, o_sd, o_ss, o_w, o_cdf, o_om;  // inside a ray block
+    int off_dec, off_feat, off_ray, off_part, off_scal, total_floats;
+    RayBlock ray;
 };
 
 
@@ -264,18 +264,8 @@ __host__ __device__ inline RenderLayout make_layout(int RT, int Sc, int Sf, int 
     L.off_dec = o; o += n_nets * kNetFloats;
     o = round_up(o, 32);
     L.off_feat = o; o += RT * L.S * kC;
-    int r = 0;
-    L.o_dC = r; r += round_up(Sc, 4);
-    L.o_sC = r; r += round_up(Sc, 4);
-    L.o_dF = r; r += round_up(Sf, 4);
-    L.o_sF = r; r += round_up(Sf, 4);
-    L.o_sd = r; r += round_up(L.S, 4);
-    L.o_ss = r; r += round_up(L.S, 4);
-    L.o_w = r; r += round_up(L.S, 4);
-    L.o_cdf = r; r += round_up(Sc, 4);
-    L.o_om = r; r += round_up(Sc, 4);
-    L.ray_stride = r;
-    L.off_ray = o; o += RT * r;
+    L.ray = make_ray_block(Sc, Sf);
+    L.off_ray = o; o += RT * L.ray.stride;
     L.off_part = o; o += RT * (L.NGc + L.NGf) * (kOut * n_nets);
     L.off_scal = o; o += 4 * RT + 4;
     L.total_floats = o;
@@ -292,6 +282,7 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
     extern __shared__ __align__(16) float smem[];
     const p3d_render_args_t& a = P.a;
     const RenderLayout& L = P.L;
+    const RayBlock& B = L.ray;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int RT = L.RT, Sc = L.Sc, Sf = L.Sf, S = L.S;
     const int n_nets = a.n_nets;
@@ -300,7 +291,7 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
     float* feat = smem + L.off_feat;
     float* rayb = smem + L.off_ray;
     float* part = smem + L.off_part;
-    float* scal = smem + L.off_scal;  // per ray: [0]=sum_w, [1]=depth ; tail: CTA min/max keys
+    float* scal = smem + L.off_scal;  // per ray: [0] = sum of the weights, [1] = monotone flag; tail: CTA min/max keys
     uint32_t* cta_keys = reinterpret_cast<uint32_t*>(scal + 4 * RT);
 
     // decoder weights -> shared memory (once per CTA)
@@ -325,30 +316,26 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
         // image of the ray -> plane set it gathers from (p3d_render_args_t::plane_index: V views of one resident plane set)
         const int bC = vC ? plane_set(a, gC / a.R) : 0, bF = vF ? plane_set(a, gF / a.R) : 0;
         const int rowC = rC * Sc + sC, rowF = RT * Sc + rF * Sf + sF;
-        float* rbC = rayb + (rC < RT ? rC : 0) * L.ray_stride;
-        float* rbF = rayb + (rF < RT ? rF : 0) * L.ray_stride;
+        float* rbC = rayb + (rC < RT ? rC : 0) * B.stride;
+        float* rbF = rayb + (rF < RT ? rF : 0) * B.stride;
 
         // ---- P1: coarse gather ------------------------------------------------------------
         float dC = 0.f;
         {
-            float px = 0.f, py = 0.f, pz = 0.f;
+            float3 p = make_float3(0.f, 0.f, 0.f);
             if (vC) {
                 dC = coarse_depth(a, gC, sC, Sc);
-                const float* o = a.ray_origins + (size_t)gC * 3;
-                const float* d = a.ray_dirs + (size_t)gC * 3;
-                px = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 0), __fmul_rn(dC, __ldg(d + 0))));
-                py = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 1), __fmul_rn(dC, __ldg(d + 1))));
-                pz = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 2), __fmul_rn(dC, __ldg(d + 2))));
+                p = sample_point(a.coord_scale, ldg3(a.ray_origins + (size_t)gC * 3), ldg3(a.ray_dirs + (size_t)gC * 3), dC);
             }
-            warp_gather(a.planes_nhwc, a.H, a.W, feat, vC ? rowC : -1, bC, px, py, pz, lane);
+            warp_gather(a.planes_nhwc, a.H, a.W, feat, vC ? rowC : -1, bC, p.x, p.y, p.z, lane);
         }
         // ---- P2: coarse sigma --------------------------------------------------------------
         if (vC) {
             float h[kHid];
             mlp_hidden(net_sigma, feat, rowC, h);
             float sg = mlp_sigma(net_sigma, h);
-            rbC[L.o_dC + sC] = dC;
-            rbC[L.o_sC + sC] = sg;
+            rbC[B.o_dC + sC] = dC;
+            rbC[B.o_sC + sC] = sg;
         }
         __syncthreads();
 
@@ -356,95 +343,40 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
         if (Sf > 0) {
             for (int r = warp; r < RT; r += nwarps) {
                 if (ray0 + r >= P.total_rays) continue;
-                float* rb = rayb + r * L.ray_stride;
-                float sw, swd;
-                warp_march(rb + L.o_dC, rb + L.o_sC, Sc, rb + L.o_w, lane, sw, swd);
-                __syncwarp();
-                if (a.dbg_weights_coarse) {
-                    float* o = a.dbg_weights_coarse + (size_t)(ray0 + r) * (Sc - 1);
-                    for (int i = lane; i < Sc - 1; i += 32) o[i] = rb[L.o_w + i];
-                }
-                warp_importance_cdf(rb + L.o_w, Sc, rb + L.o_om, rb + L.o_cdf, lane);
+                warp_coarse_pass(a, B, rayb + r * B.stride, ray0 + r, Sc, &scal[4 * r + 1], lane);
             }
             __syncthreads();
 
             // ---- P3b + P4: fine depths, gather, sigma ---------------------------------------
             float dF = 0.f;
             {
-                float px = 0.f, py = 0.f, pz = 0.f;
+                float3 p = make_float3(0.f, 0.f, 0.f);
                 if (vF) {
-                    float u = __ldg(a.u_importance + (size_t)gF * Sf + sF);
-                    int inds;
-                    dF = importance_sample(rbF + L.o_cdf, rbF + L.o_dC, Sc, u, inds);
-                    if (a.dbg_inds) a.dbg_inds[(size_t)gF * Sf + sF] = inds;
-                    if (a.dbg_depths_fine) a.dbg_depths_fine[(size_t)gF * Sf + sF] = dF;
-                    const float* o = a.ray_origins + (size_t)gF * 3;
-                    const float* d = a.ray_dirs + (size_t)gF * 3;
-                    px = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 0), __fmul_rn(dF, __ldg(d + 0))));
-                    py = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 1), __fmul_rn(dF, __ldg(d + 1))));
-                    pz = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 2), __fmul_rn(dF, __ldg(d + 2))));
+                    dF = fine_depth(a, B, rbF, gF, sF, Sc, Sf);
+                    p = sample_point(a.coord_scale, ldg3(a.ray_origins + (size_t)gF * 3), ldg3(a.ray_dirs + (size_t)gF * 3), dF);
                 }
-                warp_gather(a.planes_nhwc, a.H, a.W, feat, vF ? rowF : -1, bF, px, py, pz, lane);
+                warp_gather(a.planes_nhwc, a.H, a.W, feat, vF ? rowF : -1, bF, p.x, p.y, p.z, lane);
             }
             if (vF) {
                 float h[kHid];
                 mlp_hidden(net_sigma, feat, rowF, h);
                 float sg = mlp_sigma(net_sigma, h);
-                rbF[L.o_dF + sF] = dF;
-                rbF[L.o_sF + sF] = sg;
+                rbF[B.o_dF + sF] = dF;
+                rbF[B.o_sF + sF] = sg;
             }
             __syncthreads();
         }
 
-        // ---- P5: stable rank merge (torch.sort over cat(coarse, fine), renderer.py:157-167) ----
+        // ---- P5: stable rank merge; sample counts may be odd, so the fine depths are counted one by one ----
         int rankC = sC, rankF = 0;
-        if (vC) {
-            const float* dc = rbC + L.o_dC;
-            const float* df = rbC + L.o_dF;
-            int cnt = 0;
-            for (int i = 0; i < Sc; ++i) { float v = dc[i]; cnt += (v < dC) || (v == dC && i < sC); }
-            for (int k = 0; k < Sf; ++k) cnt += (df[k] < dC);
-            rankC = cnt;
-            rbC[L.o_sd + cnt] = dC;
-            rbC[L.o_ss + cnt] = rbC[L.o_sC + sC];
-            if (a.dbg_perm) a.dbg_perm[(size_t)gC * S + cnt] = sC;
-            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gC * S + cnt] = dC;
-        }
-        if (vF) {
-            const float* dc = rbF + L.o_dC;
-            const float* df = rbF + L.o_dF;
-            float dFv = df[sF];
-            int cnt = 0;
-            for (int i = 0; i < Sc; ++i) cnt += (dc[i] <= dFv);
-            for (int k = 0; k < Sf; ++k) { float v = df[k]; cnt += (v < dFv) || (v == dFv && k < sF); }
-            rankF = cnt;
-            rbF[L.o_sd + cnt] = dFv;
-            rbF[L.o_ss + cnt] = rbF[L.o_sF + sF];
-            if (a.dbg_perm) a.dbg_perm[(size_t)gF * S + cnt] = Sc + sF;
-            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gF * S + cnt] = dFv;
-        }
+        if (vC) rankC = merge_rank_coarse<false>(a, B, rbC, Sf > 0 && scal[4 * rC + 1] != 0.f, gC, sC, dC, Sc, Sf);
+        if (vF) rankF = merge_rank_fine<false>(a, B, rbF, scal[4 * rF + 1] != 0.f, gF, sF, Sc, Sf);
         __syncthreads();
 
         // ---- P5b: final march (warp per ray) -----------------------------------------------
         for (int r = warp; r < RT; r += nwarps) {
             if (ray0 + r >= P.total_rays) continue;
-            float* rb = rayb + r * L.ray_stride;
-            float sw, swd;
-            warp_march(rb + L.o_sd, rb + L.o_ss, S, rb + L.o_w, lane, sw, swd);
-            if (lane == 0) {
-                rb[L.o_w + S - 1] = 0.f;
-                scal[4 * r + 0] = sw;
-                float depth = __fdiv_rn(swd, sw);          // NaN when sw == 0; resolved by the clamp pass
-                a.out_depth[ray0 + r] = depth;
-                a.out_wsum[ray0 + r] = sw;
-                atomicMax(&cta_keys[0], float_to_key(rb[L.o_sd + S - 1]));   // max depth
-                atomicMax(&cta_keys[1], ~float_to_key(rb[L.o_sd]));          // min depth (complemented)
-            }
-            __syncwarp();
-            if (a.dbg_weights_final) {
-                float* o = a.dbg_weights_final + (size_t)(ray0 + r) * (S - 1);
-                for (int i = lane; i < S - 1; i += 32) o[i] = rb[L.o_w + i];
-            }
+            warp_final_pass(a, B, rayb + r * B.stride, ray0 + r, S, &scal[4 * r + 0], cta_keys, lane);
         }
         __syncthreads();
 
@@ -462,8 +394,8 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
             const int grp = pass == 0 ? sC / L.gc : L.NGc + sF / L.gf;
             float coef = 0.f;
             if (v) {
-                float wl = rank > 0 ? rb[L.o_w + rank - 1] : 0.f;
-                float wr = rb[L.o_w + rank];  // w[S-1] was zeroed
+                float wl = rank > 0 ? rb[B.o_w + rank - 1] : 0.f;
+                float wr = rb[B.o_w + rank];  // w[S-1] was zeroed
                 coef = 0.5f * (wl + wr);
             }
 #pragma unroll 1
@@ -499,44 +431,10 @@ __global__ void __launch_bounds__(256, 2) render_fwd_kernel(const RenderParams P
             }
         }
         __syncthreads();
-        {
-            const int NG = L.NGc + L.NGf;
-            for (int i = tid; i < RT * P.cout; i += blockDim.x) {
-                int r = i / P.cout, c = i % P.cout;
-                if (ray0 + r >= P.total_rays) continue;
-                const float* src = part + (size_t)r * NG * P.cout + c;
-                float acc = 0.f;
-                for (int gi = 0; gi < NG; ++gi) acc += src[gi * P.cout];
-                if (a.white_back) acc = acc + 1.f - scal[4 * r + 0];
-                a.out_feat[(size_t)(ray0 + r) * P.cout + c] = acc * 2.f - 1.f;
-            }
-        }
+        write_features(a, part, scal, ray0, RT, P.total_rays, L.NGc + L.NGf, P.cout, tid, blockDim.x);
         __syncthreads();
     }
-
-    // ---- global depth clamp: torch.clamp(depth, min(depths), max(depths)) (ray_marcher.py:49-50) ----
-    __shared__ bool is_last;
-    __threadfence();          // every thread publishes its out_depth stores before the CTA signs off
-    __syncthreads();
-    if (tid == 0) {
-        atomicMax(a.workspace + 0, cta_keys[0]);
-        atomicMax(a.workspace + 1, cta_keys[1]);
-        __threadfence();
-        unsigned done = atomicAdd(a.workspace + 2, 1u);
-        is_last = (done == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (is_last) {
-        __threadfence();
-        float dmax = key_to_float(atomicMax(a.workspace + 0, 0u));
-        float dmin = key_to_float(~atomicMax(a.workspace + 1, 0u));
-        for (int i = tid; i < P.total_rays; i += blockDim.x) {
-            float v = __ldcg(a.out_depth + i);
-            if (v != v) v = __int_as_float(0x7f800000);   // nan_to_num(nan=inf)
-            v = fminf(fmaxf(v, dmin), dmax);
-            a.out_depth[i] = v;
-        }
-    }
+    global_depth_clamp(a.workspace, cta_keys, a.out_depth, P.total_rays, blockDim.x);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -675,27 +573,7 @@ __global__ void __launch_bounds__(128) ray_march_kernel(const float* __restrict_
         kmin = max(kmin, __shfl_xor_sync(0xffffffffu, kmin, o));
     }
     if (lane == 0) { atomicMax(&keys[0], kmax); atomicMax(&keys[1], kmin); }
-    __threadfence();
-    __syncthreads();
-    __shared__ bool is_last;
-    if (threadIdx.x == 0) {
-        atomicMax(workspace + 0, keys[0]);
-        atomicMax(workspace + 1, keys[1]);
-        __threadfence();
-        unsigned done = atomicAdd(workspace + 2, 1u);
-        is_last = (done == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (is_last) {
-        __threadfence();
-        float dmax = key_to_float(atomicMax(workspace + 0, 0u));
-        float dmin = key_to_float(~atomicMax(workspace + 1, 0u));
-        for (int i = threadIdx.x; i < N; i += blockDim.x) {
-            float v = __ldcg(out_depth + i);
-            if (v != v) v = __int_as_float(0x7f800000);
-            out_depth[i] = fminf(fmaxf(v, dmin), dmax);
-        }
-    }
+    global_depth_clamp(workspace, keys, out_depth, N, blockDim.x);
 }
 
 __global__ void __launch_bounds__(128) sample_importance_kernel(const float* __restrict__ z_vals, const float* __restrict__ weights,
@@ -797,18 +675,11 @@ int p3d_pack_decoder(const p3d_decoder_t* dec, float* packed, p3d_stream_t strea
 int p3d_render_fwd(const p3d_render_args_t* args, p3d_stream_t stream) {
     if (!args) return P3D_BAD_ARG;
     const p3d_render_args_t& a = *args;
-    if (!a.planes_nhwc || !a.ray_origins || !a.ray_dirs || !depth_args_ok(a) || !a.decoder_packed || !a.out_feat ||
-        !a.out_depth || !a.out_wsum || !a.workspace)
-        return P3D_BAD_ARG;
+    if (const int st = render_args_status(a)) return st;
     if (a.plane_strides[0] || a.plane_strides[1] || a.plane_strides[2]) {
         const int64_t psz = (int64_t)a.H * a.W * kC;
         if (a.plane_strides[0] != 3 * psz || a.plane_strides[1] != psz || a.plane_strides[2] != kC) return P3D_UNSUPPORTED;
     }
-    if (a.B <= 0 || a.R <= 0 || a.H <= 0 || a.W <= 0 || a.Sc < 2 || a.Sf < 0) return P3D_BAD_ARG;
-    if (a.Sf > 0 && (!a.u_importance || a.Sc < 4)) return P3D_BAD_ARG;
-    if (a.n_nets < 1 || a.n_nets > 2 || a.sigma_net < 0 || a.sigma_net >= a.n_nets) return P3D_BAD_ARG;
-    if (a.Sc + a.Sf > 32 * kMaxIvPerLane) return P3D_UNSUPPORTED;
-    if ((int64_t)a.B * a.R > INT32_MAX / (a.Sc + a.Sf + 1)) return P3D_UNSUPPORTED;
 
     int dev = 0, max_smem = 0;
     P3D_CUDA_TRY(cudaGetDevice(&dev));

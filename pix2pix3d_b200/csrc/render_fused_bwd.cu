@@ -53,14 +53,10 @@ __host__ inline RbLayout make_rb_layout(int S, int n_nets) {
 
 // 12 bilinear taps of one sample (plane 0 <- (x, y), 1 <- (x, z), 2 <- (z, x); render_common.cuh)
 __device__ __forceinline__ void sample_taps(const p3d_render_bwd_args_t& a, int g, float dv, Taps (&t)[3]) {
-    const float* o = a.ray_origins + (size_t)g * 3;
-    const float* d = a.ray_dirs + (size_t)g * 3;
-    const float px = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 0), __fmul_rn(dv, __ldg(d + 0))));
-    const float py = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 1), __fmul_rn(dv, __ldg(d + 1))));
-    const float pz = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 2), __fmul_rn(dv, __ldg(d + 2))));
-    t[0] = make_taps(px, py, a.H, a.W);
-    t[1] = make_taps(px, pz, a.H, a.W);
-    t[2] = make_taps(pz, px, a.H, a.W);
+    const float3 p = sample_point(a.coord_scale, ldg3(a.ray_origins + (size_t)g * 3), ldg3(a.ray_dirs + (size_t)g * 3), dv);
+    t[0] = make_taps(p.x, p.y, a.H, a.W);
+    t[1] = make_taps(p.x, p.z, a.H, a.W);
+    t[2] = make_taps(p.z, p.x, a.H, a.W);
 }
 
 // channels 4q..4q+3 of one plane's bilinear sample, in tap_fetch's order

@@ -57,8 +57,8 @@ __global__ void pack_decoder_tc_kernel(PackTcArgs a, uint8_t* __restrict__ out) 
 // ---- shared-memory plan ----------------------------------------------------------------------------------
 struct TcLayout {
     int RT, Sc, Sf, S, gc, gf, NGc, NGf, tiles_c, tiles_f;
-    int off_feat, off_tail, off_ray, ray_stride, off_part, off_scal, total_bytes;
-    int o_dC, o_sC, o_dF, o_sF, o_sd, o_ss, o_w, o_cdf, o_om;
+    int off_feat, off_tail, off_ray, off_part, off_scal, total_bytes;
+    RayBlock ray;
 };
 
 __host__ __device__ inline TcLayout make_tc_layout(int RT, int Sc, int Sf, int n_nets) {
@@ -70,18 +70,8 @@ __host__ __device__ inline TcLayout make_tc_layout(int RT, int Sc, int Sf, int n
     int o = kTcTail;                                   // weight tiles first (1024-aligned base)
     L.off_feat = o; o += (L.tiles_c + L.tiles_f) * 16384;
     L.off_tail = o; o += kTcTailFloats * 4;
-    int r = 0;
-    L.o_dC = r; r += round_up(Sc, 4);
-    L.o_sC = r; r += round_up(Sc, 4);
-    L.o_dF = r; r += round_up(Sf, 4);
-    L.o_sF = r; r += round_up(Sf, 4);
-    L.o_sd = r; r += round_up(L.S, 4);
-    L.o_ss = r; r += round_up(L.S, 4);
-    L.o_w = r; r += round_up(L.S, 4);
-    L.o_cdf = r; r += round_up(Sc, 4);
-    L.o_om = r; r += round_up(Sc, 4);
-    L.ray_stride = r;
-    L.off_ray = o; o += RT * r * 4;
+    L.ray = make_ray_block(Sc, Sf);
+    L.off_ray = o; o += RT * L.ray.stride * 4;
     L.off_part = o; o += RT * (L.NGc + L.NGf) * (kOut * n_nets) * 4;
     L.off_scal = o; o += (4 * RT + 4) * 4;
     L.total_bytes = o;
@@ -104,6 +94,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     const p3d_render_args_t& a = P.a;
     const TcLayout& L = P.L;
+    const RayBlock& B = L.ray;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = kTcThreads >> 5;
     // group (warpgroup), row inside the group's tile, warp of the group. The group index is broadcast from lane 0 so that the
     // compiler sees it warp-uniform: the per-group branches around the decoder's wgmma are then not divergent paths, which
@@ -152,7 +143,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int i = grp * 128 + dec_frag_row(mb, h, q, lane), r = i / n;
-                    if (r < RT && ray0 + r < P.total_rays) rayb[r * L.ray_stride + o_s + i % n] = sg[mb][h];
+                    if (r < RT && ray0 + r < P.total_rays) rayb[r * B.stride + o_s + i % n] = sg[mb][h];
                 }
         }
     };
@@ -168,27 +159,23 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
         const int gC = ray0 + rC, gF = ray0 + rF;
         // image of the ray -> plane set it gathers from (p3d_render_args_t::plane_index: V views of one resident plane set)
         const int bC = vC ? plane_set(a, gC / a.R) : 0, bF = vF ? plane_set(a, gF / a.R) : 0;
-        float* rbC = rayb + (rC < RT ? rC : 0) * L.ray_stride;
-        float* rbF = rayb + (rF < RT ? rF : 0) * L.ray_stride;
+        float* rbC = rayb + (rC < RT ? rC : 0) * B.stride;
+        float* rbF = rayb + (rF < RT ? rF : 0) * B.stride;
         const bool grpC = grp < L.tiles_c, grpF = grp < L.tiles_f;   // does this group own a coarse / fine tile?
 
         // ---- P1/P2: coarse gather + sigma -------------------------------------------------------------
         float dC = 0.f;
         if (grpC) {
-            float px = 0.f, py = 0.f, pz = 0.f;
+            float3 p = make_float3(0.f, 0.f, 0.f);
             if (vC) {
                 dC = coarse_depth(a, gC, sC, Sc);
-                const float* o = a.ray_origins + (size_t)gC * 3;
-                const float* d = a.ray_dirs + (size_t)gC * 3;
-                px = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 0), __fmul_rn(dC, __ldg(d + 0))));
-                py = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 1), __fmul_rn(dC, __ldg(d + 1))));
-                pz = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 2), __fmul_rn(dC, __ldg(d + 2))));
+                p = sample_point(a.coord_scale, ldg3(a.ray_origins + (size_t)gC * 3), ldg3(a.ray_dirs + (size_t)gC * 3), dC);
             }
-            gather_rows(grp, vC, bC, px, py, pz);
+            gather_rows(grp, vC, bC, p.x, p.y, p.z);
             tc::fence_proxy_async();
             group_sync();
-            density(grp, Sc, L.o_sC, ray0);
-            if (vC) rbC[L.o_dC + sC] = dC;
+            density(grp, Sc, B.o_sC, ray0);
+            if (vC) rbC[B.o_dC + sC] = dC;
         }
         __syncthreads();
 
@@ -197,115 +184,36 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
         if (Sf > 0) {
             for (int r = warp; r < RT; r += nwarps) {
                 if (ray0 + r >= P.total_rays) continue;
-                float* rb = rayb + r * L.ray_stride;
-                float sw, swd;
-                warp_march(rb + L.o_dC, rb + L.o_sC, Sc, rb + L.o_w, lane, sw, swd);
-                __syncwarp();
-                if (a.dbg_weights_coarse) {
-                    float* o = a.dbg_weights_coarse + (size_t)(ray0 + r) * (Sc - 1);
-                    for (int i = lane; i < Sc - 1; i += 32) o[i] = rb[L.o_w + i];
-                }
-                warp_importance_cdf(rb + L.o_w, Sc, rb + L.o_om, rb + L.o_cdf, lane);
-                // stratified depths are non-decreasing by construction (renderer.py:169-192); when they are, the merge below
-                // knows a coarse sample's rank among the coarse ones (its index) and can binary-search them
-                bool mono = true;
-                for (int i = lane; i < Sc - 1; i += 32) mono = mono && (rb[L.o_dC + i] <= rb[L.o_dC + i + 1]);
-                mono = __all_sync(0xffffffffu, mono);
-                if (lane == 0) scal[4 * r + 1] = mono ? 1.f : 0.f;
+                warp_coarse_pass(a, B, rayb + r * B.stride, ray0 + r, Sc, &scal[4 * r + 1], lane);
             }
             __syncthreads();
 
             // ---- P3b/P4: fine depths, gather, sigma ----------------------------------------------------
             if (grpF) {
-                float px = 0.f, py = 0.f, pz = 0.f;
+                float3 p = make_float3(0.f, 0.f, 0.f);
                 if (vF) {
-                    const float u = __ldg(a.u_importance + (size_t)gF * Sf + sF);
-                    int inds;
-                    dF = importance_sample(rbF + L.o_cdf, rbF + L.o_dC, Sc, u, inds);
-                    if (a.dbg_inds) a.dbg_inds[(size_t)gF * Sf + sF] = inds;
-                    if (a.dbg_depths_fine) a.dbg_depths_fine[(size_t)gF * Sf + sF] = dF;
-                    const float* o = a.ray_origins + (size_t)gF * 3;
-                    const float* d = a.ray_dirs + (size_t)gF * 3;
-                    px = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 0), __fmul_rn(dF, __ldg(d + 0))));
-                    py = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 1), __fmul_rn(dF, __ldg(d + 1))));
-                    pz = __fmul_rn(a.coord_scale, __fadd_rn(__ldg(o + 2), __fmul_rn(dF, __ldg(d + 2))));
+                    dF = fine_depth(a, B, rbF, gF, sF, Sc, Sf);
+                    p = sample_point(a.coord_scale, ldg3(a.ray_origins + (size_t)gF * 3), ldg3(a.ray_dirs + (size_t)gF * 3), dF);
                 }
-                gather_rows(L.tiles_c + grp, vF, bF, px, py, pz);
+                gather_rows(L.tiles_c + grp, vF, bF, p.x, p.y, p.z);
                 tc::fence_proxy_async();
                 group_sync();
-                density(L.tiles_c + grp, Sf, L.o_sF, ray0);
-                if (vF) rbF[L.o_dF + sF] = dF;
+                density(L.tiles_c + grp, Sf, B.o_sF, ray0);
+                if (vF) rbF[B.o_dF + sF] = dF;
             }
             __syncthreads();
         }
 
-        // ---- P5: stable rank merge (renderer.py:157-167) -------------------------------------------------
+        // ---- P5: stable rank merge ---------------------------------------------------------------------------------
         int rankC = sC, rankF = 0;
-        if (vC && grpC) {
-            const float* dc = rbC + L.o_dC;
-            const float* df = rbC + L.o_dF;
-            int cnt = 0;
-            if (Sf > 0 && scal[4 * rC + 1] != 0.f) cnt = sC;
-            else for (int i = 0; i < Sc; ++i) { float v = dc[i]; cnt += (v < dC) || (v == dC && i < sC); }
-            // sample counts are multiples of 8 and the per-ray arrays 16-byte aligned: four depths per LDS.128
-            const float4* df4 = reinterpret_cast<const float4*>(df);
-            for (int k = 0; k < (Sf >> 2); ++k) {
-                const float4 f = df4[k];
-                cnt += (f.x < dC) + (f.y < dC) + (f.z < dC) + (f.w < dC);
-            }
-            rankC = cnt;
-            rbC[L.o_sd + cnt] = dC;
-            rbC[L.o_ss + cnt] = rbC[L.o_sC + sC];
-            if (a.dbg_perm) a.dbg_perm[(size_t)gC * S + cnt] = sC;
-            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gC * S + cnt] = dC;
-        }
-        if (vF && grpF) {
-            const float* dc = rbF + L.o_dC;
-            const float* df = rbF + L.o_dF;
-            const float dFv = df[sF];
-            int cnt = 0;
-            if (scal[4 * rF + 1] != 0.f) {
-                int lo = 0, hi = Sc;                         // upper bound: number of coarse depths <= dFv
-                while (lo < hi) { const int mid = (lo + hi) >> 1; if (dc[mid] <= dFv) lo = mid + 1; else hi = mid; }
-                cnt = lo;
-            } else {
-                for (int i = 0; i < Sc; ++i) cnt += (dc[i] <= dFv);
-            }
-            // stable rank among the fine samples: #(v < d) over all + #(v == d) over the earlier ones
-            const float4* df4 = reinterpret_cast<const float4*>(df);
-            for (int k = 0; k < (Sf >> 2); ++k) {
-                const float4 f = df4[k];
-                const int k0 = 4 * k;
-                cnt += (f.x < dFv) + (f.y < dFv) + (f.z < dFv) + (f.w < dFv);
-                cnt += ((f.x == dFv) & (k0 < sF)) + ((f.y == dFv) & (k0 + 1 < sF)) + ((f.z == dFv) & (k0 + 2 < sF)) + ((f.w == dFv) & (k0 + 3 < sF));
-            }
-            rankF = cnt;
-            rbF[L.o_sd + cnt] = dFv;
-            rbF[L.o_ss + cnt] = rbF[L.o_sF + sF];
-            if (a.dbg_perm) a.dbg_perm[(size_t)gF * S + cnt] = Sc + sF;
-            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gF * S + cnt] = dFv;
-        }
+        if (vC && grpC) rankC = merge_rank_coarse<true>(a, B, rbC, Sf > 0 && scal[4 * rC + 1] != 0.f, gC, sC, dC, Sc, Sf);
+        if (vF && grpF) rankF = merge_rank_fine<true>(a, B, rbF, scal[4 * rF + 1] != 0.f, gF, sF, Sc, Sf);
         __syncthreads();
 
         // ---- P5b: final march ---------------------------------------------------------------------------
         for (int r = warp; r < RT; r += nwarps) {
             if (ray0 + r >= P.total_rays) continue;
-            float* rb = rayb + r * L.ray_stride;
-            float sw, swd;
-            warp_march(rb + L.o_sd, rb + L.o_ss, S, rb + L.o_w, lane, sw, swd);
-            if (lane == 0) {
-                rb[L.o_w + S - 1] = 0.f;
-                scal[4 * r + 0] = sw;
-                a.out_depth[ray0 + r] = __fdiv_rn(swd, sw);
-                a.out_wsum[ray0 + r] = sw;
-                atomicMax(&cta_keys[0], float_to_key(rb[L.o_sd + S - 1]));
-                atomicMax(&cta_keys[1], ~float_to_key(rb[L.o_sd]));
-            }
-            __syncwarp();
-            if (a.dbg_weights_final) {
-                float* o = a.dbg_weights_final + (size_t)(ray0 + r) * (S - 1);
-                for (int i = lane; i < S - 1; i += 32) o[i] = rb[L.o_w + i];
-            }
+            warp_final_pass(a, B, rayb + r * B.stride, ray0 + r, S, &scal[4 * r + 0], cta_keys, lane);
         }
         __syncthreads();
 
@@ -323,8 +231,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
             const int slot = pass == 0 ? sC / L.gc : L.NGc + sF / L.gf;
             float coef = 0.f;
             if (v) {
-                const float wl = rank > 0 ? rb[L.o_w + rank - 1] : 0.f;
-                coef = 0.5f * (wl + rb[L.o_w + rank]);
+                const float wl = rank > 0 ? rb[B.o_w + rank - 1] : 0.f;
+                coef = 0.5f * (wl + rb[B.o_w + rank]);
             }
             // colour pre-activations of one net (this thread's row) -> bias, sigmoid where masked, x coefficient,
             // reduction over the rows of a ray segment -> per-segment partial sums in shared memory
@@ -353,34 +261,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
                     for (int i = 0; i < 32; ++i) acc[i] = 0.f;     // rows beyond the tile's rays may hold NaN garbage: coef 0 is not enough
                 }
                 float* dst = part + ((size_t)(rr < RT ? rr : 0) * (L.NGc + L.NGf) + slot) * P.cout + net * kOut;
-                if (g == 16) {
-                    // transposed butterfly over the 16 lanes of a ray segment: every step halves the channels a lane keeps
-                    // (30 shuffles instead of 128); lane ends with the two channels [base, base + 2)
-                    int base = 0;
-#define P3D_RED_STEP(O, N)                                                                         \
-    {                                                                                              \
-        const bool up = (lane & O) != 0;                                                           \
-        _Pragma("unroll") for (int i = 0; i < N / 2; ++i) {                                        \
-            const float send = up ? acc[i] : acc[i + N / 2];                                       \
-            const float keep = up ? acc[i + N / 2] : acc[i];                                       \
-            acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, O);                                 \
-        }                                                                                          \
-        base += up ? N / 2 : 0;                                                                    \
-    }
-                    P3D_RED_STEP(8, 32) P3D_RED_STEP(4, 16) P3D_RED_STEP(2, 8) P3D_RED_STEP(1, 4)
-#undef P3D_RED_STEP
-                    if (rr < RT) *reinterpret_cast<float2*>(dst + base) = make_float2(acc[0], acc[1]);
-                } else {
-                    for (int o = g >> 1; o > 0; o >>= 1) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
-                    }
-                    if ((lane & (g - 1)) == 0 && rr < RT) {
-#pragma unroll
-                        for (int i = 0; i < 32; i += 4)
-                            *reinterpret_cast<float4*>(dst + i) = make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
-                    }
-                }
+                segment_sum32(acc, g, lane, rr < RT, dst);
             };
             // colour pre-activations of both nets from this pass's feature tile, then the tile is their staging area
             uint8_t* ftile = feat + ((pass == 0 ? 0 : L.tiles_c) + grp) * 16384;
@@ -406,43 +287,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) render_fwd_tc_kernel(const TcRe
             }
         }
         __syncthreads();
-        {
-            const int NG = L.NGc + L.NGf;
-            for (int i = tid; i < RT * P.cout; i += kTcThreads) {
-                const int r = i / P.cout, c = i % P.cout;
-                if (ray0 + r >= P.total_rays) continue;
-                const float* src = part + (size_t)r * NG * P.cout + c;
-                float acc = 0.f;
-                for (int gi = 0; gi < NG; ++gi) acc += src[gi * P.cout];
-                if (a.white_back) acc = acc + 1.f - scal[4 * r + 0];
-                a.out_feat[(size_t)(ray0 + r) * P.cout + c] = acc * 2.f - 1.f;
-            }
-        }
+        write_features(a, part, scal, ray0, RT, P.total_rays, L.NGc + L.NGf, P.cout, tid, kTcThreads);
         __syncthreads();
     }
-
-    // ---- global depth clamp (ray_marcher.py:49-50) -----------------------------------------------------------
-    __shared__ bool is_last;
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) {
-        atomicMax(a.workspace + 0, cta_keys[0]);
-        atomicMax(a.workspace + 1, cta_keys[1]);
-        __threadfence();
-        const unsigned done = atomicAdd(a.workspace + 2, 1u);
-        is_last = (done == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (is_last) {
-        __threadfence();
-        const float dmax = key_to_float(atomicMax(a.workspace + 0, 0u));
-        const float dmin = key_to_float(~atomicMax(a.workspace + 1, 0u));
-        for (int i = tid; i < P.total_rays; i += kTcThreads) {
-            float v = __ldcg(a.out_depth + i);
-            if (v != v) v = __int_as_float(0x7f800000);
-            a.out_depth[i] = fminf(fmaxf(v, dmin), dmax);
-        }
-    }
+    global_depth_clamp(a.workspace, cta_keys, a.out_depth, P.total_rays, kTcThreads);
 }
 
 }  // namespace p3d
@@ -467,14 +315,8 @@ extern "C" int p3d_pack_decoder_tc(const p3d_decoder_t* dec, void* packed, p3d_s
 extern "C" int p3d_render_fwd_tc(const p3d_render_args_t* args, p3d_stream_t stream) {
     if (!args) return P3D_BAD_ARG;
     const p3d_render_args_t& a = *args;
-    if (!a.planes_nhwc || !a.ray_origins || !a.ray_dirs || !depth_args_ok(a) || !a.decoder_packed || !a.out_feat ||
-        !a.out_depth || !a.out_wsum || !a.workspace)
-        return P3D_BAD_ARG;
-    if (a.B <= 0 || a.R <= 0 || a.H <= 0 || a.W <= 0 || a.Sc < 2 || a.Sf < 0) return P3D_BAD_ARG;
-    if (a.Sf > 0 && (!a.u_importance || a.Sc < 4)) return P3D_BAD_ARG;
-    if (a.n_nets < 1 || a.n_nets > 2 || a.sigma_net < 0 || a.sigma_net >= a.n_nets) return P3D_BAD_ARG;
-    if ((a.Sc % 8) || (a.Sf % 8) || a.Sc > 128 || a.Sf > 128 || a.Sc + a.Sf > 32 * kMaxIvPerLane) return P3D_UNSUPPORTED;
-    if ((int64_t)a.B * a.R > INT32_MAX / (a.Sc + a.Sf + 1)) return P3D_UNSUPPORTED;
+    if (const int st = render_args_status(a)) return st;
+    if ((a.Sc % 8) || (a.Sf % 8) || a.Sc > 128 || a.Sf > 128) return P3D_UNSUPPORTED;
 
     int dev = 0, max_smem = 0;
     P3D_CUDA_TRY(cudaGetDevice(&dev));
@@ -493,18 +335,9 @@ extern "C" int p3d_render_fwd_tc(const p3d_render_args_t* args, p3d_stream_t str
     P.total_rays = a.B * a.R;
     P.n_tiles = ceil_div(P.total_rays, RT);
     P.cout = kOut * a.n_nets;
-    {
-        const int64_t psz = (int64_t)a.H * a.W * kC;
-        const bool dense = !(a.plane_strides[0] || a.plane_strides[1] || a.plane_strides[2]);
-        const int64_t is = dense ? 3 * psz : a.plane_strides[0], pls = dense ? psz : a.plane_strides[1], pxs = dense ? kC : a.plane_strides[2];
-        if (is <= 0 || pls <= 0 || pxs < kC) return P3D_BAD_ARG;
-        // 16-byte texel vectors: base and strides must keep every 4-channel group aligned
-        if ((((uintptr_t)a.planes_nhwc) & 15) != 0 || (is & 3) || (pls & 3) || (pxs & 3)) return P3D_UNSUPPORTED;
-        // largest element offset the kernel forms must fit 32 bits
-        const int64_t max_off = (int64_t)(a.B - 1) * is + 2 * pls + ((int64_t)a.H * a.W - 1) * pxs + kC;
-        if (max_off >= ((int64_t)1 << 32)) return P3D_UNSUPPORTED;
-        P.img_stride = (uint32_t)is; P.plane_stride = (uint32_t)pls; P.pix_stride = (uint32_t)pxs;
-    }
+    if (const int st = plane_strides_status(a.planes_nhwc, a.plane_strides, a.B, a.H, a.W, P.img_stride, P.plane_stride,
+                                            P.pix_stride))
+        return st;
     {
         // args.tc_variant = 1 selects the ray-pair variant (render_tc2.cu)
         if (a.tc_variant == 1 && (a.Sc > 64 || a.Sf > 64)) return P3D_UNSUPPORTED;

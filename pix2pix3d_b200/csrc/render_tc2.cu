@@ -14,7 +14,7 @@ namespace p3d {
 
 struct PairLayout {
     int Sc, Sf, S, gc, gf, NGc, NGf, cout;
-    int ray_stride, o_dC, o_sC, o_dF, o_sF, o_sd, o_ss, o_w, o_cdf, o_om;
+    RayBlock ray;
     int grp_bytes, g_feat, g_ray, g_part, g_scal;      // offsets inside a group's block
     int off_tail, off_groups, total_bytes;
 };
@@ -24,20 +24,10 @@ __host__ __device__ inline PairLayout make_pair_layout(int Sc, int Sf, int n_net
     L.Sc = Sc; L.Sf = Sf; L.S = Sc + Sf; L.cout = kOut * n_nets;
     L.gc = pow2_group(Sc); L.gf = Sf > 0 ? pow2_group(Sf) : 1;
     L.NGc = Sc / L.gc; L.NGf = Sf > 0 ? Sf / L.gf : 0;
-    int r = 0;
-    L.o_dC = r; r += round_up(Sc, 4);
-    L.o_sC = r; r += round_up(Sc, 4);
-    L.o_dF = r; r += round_up(Sf, 4);
-    L.o_sF = r; r += round_up(Sf, 4);
-    L.o_sd = r; r += round_up(L.S, 4);
-    L.o_ss = r; r += round_up(L.S, 4);
-    L.o_w = r; r += round_up(L.S, 4);
-    L.o_cdf = r; r += round_up(Sc, 4);
-    L.o_om = r; r += round_up(Sc, 4);
-    L.ray_stride = r;
+    L.ray = make_ray_block(Sc, Sf);
     int g = 0;
     L.g_feat = g; g += 2 * 16384;                       // coarse tile, fine tile (1024-aligned: groups start aligned)
-    L.g_ray = g; g += 2 * r * 4;
+    L.g_ray = g; g += 2 * L.ray.stride * 4;
     L.g_part = g; g += 2 * (L.NGc + L.NGf) * L.cout * 4;
     L.g_scal = g; g += 8 * 4;                            // per ray: weight sum, monotone flag
     L.grp_bytes = round_up(g, 1024);
@@ -62,6 +52,7 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     const p3d_render_args_t& a = P.a;
     const PairLayout& L = P.L;
+    const RayBlock& B = L.ray;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int grp = tid >> 7, m = tid & 127, q = warp & 3;
     const int Sc = L.Sc, Sf = L.Sf, S = L.S, n_nets = a.n_nets, cout = L.cout;
@@ -105,7 +96,7 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int s_r = dec_frag_row(mb, h, q, lane) & 63;
-                    if (pair * 2 + mb < P.total_rays && s_r < n) rayb[mb * L.ray_stride + o_s + s_r] = sg[mb][h];
+                    if (pair * 2 + mb < P.total_rays && s_r < n) rayb[mb * B.stride + o_s + s_r] = sg[mb][h];
                 }
         }
     };
@@ -115,30 +106,26 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
         const bool rvalid = gray < P.total_rays;
         const bool vC = rvalid && sidx < Sc, vF = rvalid && Sf > 0 && sidx < Sf;
         const int b = rvalid ? plane_set(a, gray / a.R) : 0;
-        float* rb = rayb + half * L.ray_stride;
-        float ox = 0.f, oy = 0.f, oz = 0.f, dx = 0.f, dy = 0.f, dz = 0.f;
+        float* rb = rayb + half * B.stride;
+        float3 ro = make_float3(0.f, 0.f, 0.f), rd = ro;
         if (rvalid) {
-            const float* o = a.ray_origins + (size_t)gray * 3;
-            const float* d = a.ray_dirs + (size_t)gray * 3;
-            ox = __ldg(o + 0); oy = __ldg(o + 1); oz = __ldg(o + 2);
-            dx = __ldg(d + 0); dy = __ldg(d + 1); dz = __ldg(d + 2);
+            ro = ldg3(a.ray_origins + (size_t)gray * 3);
+            rd = ldg3(a.ray_dirs + (size_t)gray * 3);
         }
 
         // ---- A: coarse gather + density ---------------------------------------------------------------------
         float dC = 0.f;
         {
-            float px = 0.f, py = 0.f, pz = 0.f;
+            float3 p = make_float3(0.f, 0.f, 0.f);
             if (vC) {
                 dC = coarse_depth(a, gray, sidx, Sc);
-                px = __fmul_rn(a.coord_scale, __fadd_rn(ox, __fmul_rn(dC, dx)));
-                py = __fmul_rn(a.coord_scale, __fadd_rn(oy, __fmul_rn(dC, dy)));
-                pz = __fmul_rn(a.coord_scale, __fadd_rn(oz, __fmul_rn(dC, dz)));
+                p = sample_point(a.coord_scale, ro, rd, dC);
             }
-            tc_gather_rows(pv, feat, q, lane, vC, b, px, py, pz);
+            tc_gather_rows(pv, feat, q, lane, vC, b, p.x, p.y, p.z);
             tc::fence_proxy_async();
             group_sync();
-            density(0, Sc, L.o_sC, pair);
-            if (vC) rb[L.o_dC + sidx] = dC;
+            density(0, Sc, B.o_sC, pair);
+            if (vC) rb[B.o_dC + sidx] = dC;
         }
         group_sync();
 
@@ -147,102 +134,36 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
         if (Sf > 0) {
             if ((q & 1) == 0) {
                 const int r = q >> 1;
-                if (pair * 2 + r < P.total_rays) {
-                    float* rr = rayb + r * L.ray_stride;
-                    float sw, swd;
-                    warp_march(rr + L.o_dC, rr + L.o_sC, Sc, rr + L.o_w, lane, sw, swd);
-                    __syncwarp();
-                    if (a.dbg_weights_coarse) {
-                        float* o = a.dbg_weights_coarse + (size_t)(pair * 2 + r) * (Sc - 1);
-                        for (int i = lane; i < Sc - 1; i += 32) o[i] = rr[L.o_w + i];
-                    }
-                    warp_importance_cdf(rr + L.o_w, Sc, rr + L.o_om, rr + L.o_cdf, lane);
-                    bool mono = true;
-                    for (int i = lane; i < Sc - 1; i += 32) mono = mono && (rr[L.o_dC + i] <= rr[L.o_dC + i + 1]);
-                    mono = __all_sync(0xffffffffu, mono);
-                    if (lane == 0) scal[4 * r + 1] = mono ? 1.f : 0.f;
-                }
+                if (pair * 2 + r < P.total_rays)
+                    warp_coarse_pass(a, B, rayb + r * B.stride, pair * 2 + r, Sc, &scal[4 * r + 1], lane);
             }
             group_sync();
 
             // ---- C: fine depths, gather, density --------------------------------------------------------------
-            float px = 0.f, py = 0.f, pz = 0.f;
+            float3 p = make_float3(0.f, 0.f, 0.f);
             if (vF) {
-                const float u = __ldg(a.u_importance + (size_t)gray * Sf + sidx);
-                int inds;
-                dF = importance_sample(rb + L.o_cdf, rb + L.o_dC, Sc, u, inds);
-                if (a.dbg_inds) a.dbg_inds[(size_t)gray * Sf + sidx] = inds;
-                if (a.dbg_depths_fine) a.dbg_depths_fine[(size_t)gray * Sf + sidx] = dF;
-                px = __fmul_rn(a.coord_scale, __fadd_rn(ox, __fmul_rn(dF, dx)));
-                py = __fmul_rn(a.coord_scale, __fadd_rn(oy, __fmul_rn(dF, dy)));
-                pz = __fmul_rn(a.coord_scale, __fadd_rn(oz, __fmul_rn(dF, dz)));
+                dF = fine_depth(a, B, rb, gray, sidx, Sc, Sf);
+                p = sample_point(a.coord_scale, ro, rd, dF);
             }
-            tc_gather_rows(pv, feat + 16384, q, lane, vF, b, px, py, pz);
+            tc_gather_rows(pv, feat + 16384, q, lane, vF, b, p.x, p.y, p.z);
             tc::fence_proxy_async();
             group_sync();
-            density(1, Sf, L.o_sF, pair);
-            if (vF) rb[L.o_dF + sidx] = dF;
+            density(1, Sf, B.o_sF, pair);
+            if (vF) rb[B.o_dF + sidx] = dF;
             group_sync();
         }
 
-        // ---- D: stable rank merge (renderer.py:157-167) -----------------------------------------------------------
+        // ---- D: stable rank merge ------------------------------------------------------------------------------------
         int rankC = sidx, rankF = 0;
-        if (vC) {
-            const float* dc = rb + L.o_dC;
-            const float* df = rb + L.o_dF;
-            int cnt = 0;
-            if (Sf > 0 && scal[4 * half + 1] != 0.f) cnt = sidx;
-            else for (int i = 0; i < Sc; ++i) { const float v = dc[i]; cnt += (v < dC) || (v == dC && i < sidx); }
-            for (int k = 0; k < Sf; ++k) cnt += (df[k] < dC);
-            rankC = cnt;
-            rb[L.o_sd + cnt] = dC;
-            rb[L.o_ss + cnt] = rb[L.o_sC + sidx];
-            if (a.dbg_perm) a.dbg_perm[(size_t)gray * S + cnt] = sidx;
-            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gray * S + cnt] = dC;
-        }
-        if (vF) {
-            const float* dc = rb + L.o_dC;
-            const float* df = rb + L.o_dF;
-            const float dFv = df[sidx];
-            int cnt = 0;
-            if (scal[4 * half + 1] != 0.f) {
-                int lo = 0, hi = Sc;
-                while (lo < hi) { const int mid = (lo + hi) >> 1; if (dc[mid] <= dFv) lo = mid + 1; else hi = mid; }
-                cnt = lo;
-            } else {
-                for (int i = 0; i < Sc; ++i) cnt += (dc[i] <= dFv);
-            }
-            for (int k = 0; k < Sf; ++k) { const float v = df[k]; cnt += (v < dFv) || (v == dFv && k < sidx); }
-            rankF = cnt;
-            rb[L.o_sd + cnt] = dFv;
-            rb[L.o_ss + cnt] = rb[L.o_sF + sidx];
-            if (a.dbg_perm) a.dbg_perm[(size_t)gray * S + cnt] = Sc + sidx;
-            if (a.out_depths_sorted) a.out_depths_sorted[(size_t)gray * S + cnt] = dFv;
-        }
+        if (vC) rankC = merge_rank_coarse<true>(a, B, rb, Sf > 0 && scal[4 * half + 1] != 0.f, gray, sidx, dC, Sc, Sf);
+        if (vF) rankF = merge_rank_fine<true>(a, B, rb, scal[4 * half + 1] != 0.f, gray, sidx, Sc, Sf);
         group_sync();
 
         // ---- E: final march ---------------------------------------------------------------------------------------
         if ((q & 1) == 0) {
             const int r = q >> 1;
-            const int gr = pair * 2 + r;
-            if (gr < P.total_rays) {
-                float* rr = rayb + r * L.ray_stride;
-                float sw, swd;
-                warp_march(rr + L.o_sd, rr + L.o_ss, S, rr + L.o_w, lane, sw, swd);
-                if (lane == 0) {
-                    rr[L.o_w + S - 1] = 0.f;
-                    scal[4 * r + 0] = sw;
-                    a.out_depth[gr] = __fdiv_rn(swd, sw);
-                    a.out_wsum[gr] = sw;
-                    atomicMax(&cta_keys[0], float_to_key(rr[L.o_sd + S - 1]));
-                    atomicMax(&cta_keys[1], ~float_to_key(rr[L.o_sd]));
-                }
-                __syncwarp();
-                if (a.dbg_weights_final) {
-                    float* o = a.dbg_weights_final + (size_t)gr * (S - 1);
-                    for (int i = lane; i < S - 1; i += 32) o[i] = rr[L.o_w + i];
-                }
-            }
+            if (pair * 2 + r < P.total_rays)
+                warp_final_pass(a, B, rayb + r * B.stride, pair * 2 + r, S, &scal[4 * r + 0], cta_keys, lane);
         }
         group_sync();
 
@@ -256,8 +177,8 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
             const int slot = pass == 0 ? sidx / L.gc : L.NGc + sidx / L.gf;
             float coef = 0.f;
             if (v) {
-                const float wl = rank > 0 ? rb[L.o_w + rank - 1] : 0.f;
-                coef = 0.5f * (wl + rb[L.o_w + rank]);
+                const float wl = rank > 0 ? rb[B.o_w + rank - 1] : 0.f;
+                coef = 0.5f * (wl + rb[B.o_w + rank]);
             }
             // colour pre-activations of both nets from this pass's feature tile, then the tile is their staging area
             float d2[2][2][16];
@@ -287,75 +208,16 @@ __global__ void __launch_bounds__(kPairThreads, 1) render_fwd_tc_pairs_kernel(co
                 }
                 float* dst = part + ((size_t)half * (L.NGc + L.NGf) + slot) * cout + net * kOut;
                 const bool seg_live = (sidx - (sidx & (g - 1))) < (pass == 0 ? Sc : Sf);   // first row of this lane group exists
-                if (g == 16) {
-                    int base = 0;
-#define P3D_RED_STEP(O, N)                                                                         \
-    {                                                                                              \
-        const bool up = (lane & O) != 0;                                                           \
-        _Pragma("unroll") for (int i = 0; i < N / 2; ++i) {                                        \
-            const float send = up ? acc[i] : acc[i + N / 2];                                       \
-            const float keep = up ? acc[i + N / 2] : acc[i];                                       \
-            acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, O);                                 \
-        }                                                                                          \
-        base += up ? N / 2 : 0;                                                                    \
-    }
-                    P3D_RED_STEP(8, 32) P3D_RED_STEP(4, 16) P3D_RED_STEP(2, 8) P3D_RED_STEP(1, 4)
-#undef P3D_RED_STEP
-                    if (seg_live) *reinterpret_cast<float2*>(dst + base) = make_float2(acc[0], acc[1]);
-                } else {
-                    for (int o = g >> 1; o > 0; o >>= 1) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
-                    }
-                    if ((lane & (g - 1)) == 0 && seg_live) {
-#pragma unroll
-                        for (int i = 0; i < 32; i += 4)
-                            *reinterpret_cast<float4*>(dst + i) = make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
-                    }
-                }
+                segment_sum32(acc, g, lane, seg_live, dst);
                 group_sync();  // the staging rows are rewritten by the next net
             }
         }
         group_sync();
         // ---- G: per-ray sums of the lane-group partials ----------------------------------------------------------------
-        {
-            const int NG = L.NGc + L.NGf;
-            for (int i = m; i < 2 * cout; i += 128) {
-                const int r = i / cout, c = i - r * cout;
-                const int gr = pair * 2 + r;
-                if (gr >= P.total_rays) continue;
-                const float* src = part + (size_t)r * NG * cout + c;
-                float acc = 0.f;
-                for (int gi = 0; gi < NG; ++gi) acc += src[gi * cout];
-                if (a.white_back) acc = acc + 1.f - scal[4 * r + 0];
-                a.out_feat[(size_t)gr * cout + c] = acc * 2.f - 1.f;
-            }
-        }
+        write_features(a, part, scal, pair * 2, 2, P.total_rays, L.NGc + L.NGf, cout, m, 128);
         group_sync();
     }
-
-    // ---- global depth clamp (ray_marcher.py:49-50) ---------------------------------------------------------------
-    __shared__ bool is_last;
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) {
-        atomicMax(a.workspace + 0, cta_keys[0]);
-        atomicMax(a.workspace + 1, cta_keys[1]);
-        __threadfence();
-        const unsigned done = atomicAdd(a.workspace + 2, 1u);
-        is_last = (done == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (is_last) {
-        __threadfence();
-        const float dmax = key_to_float(atomicMax(a.workspace + 0, 0u));
-        const float dmin = key_to_float(~atomicMax(a.workspace + 1, 0u));
-        for (int i = tid; i < P.total_rays; i += kPairThreads) {
-            float v = __ldcg(a.out_depth + i);
-            if (v != v) v = __int_as_float(0x7f800000);
-            a.out_depth[i] = fminf(fmaxf(v, dmin), dmax);
-        }
-    }
+    global_depth_clamp(a.workspace, cta_keys, a.out_depth, P.total_rays, kPairThreads);
 }
 
 // Host side of the ray-pair variant; argument checks and plane strides are done by p3d_render_fwd_tc (render_tc.cu).

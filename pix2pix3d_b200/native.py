@@ -156,6 +156,18 @@ def _out_view(buf, shape, dtype, dev):
     return buf.reshape(-1)[:n].view(shape)
 
 
+def _in_place_strides(planes_nhwc):
+    """(image, plane, pixel) element strides of a non-contiguous [B,3,H,W,32] plane view that the tensor-core kernels read in
+    place: channels contiguous and rows W pixels apart (e.g. the backbone's NHWC [B,H,W,96] output viewed as
+    [B,3,H,W,32]). None for a contiguous tensor and for any other view, which is made dense first."""
+    if planes_nhwc.is_contiguous():
+        return None
+    st_img, st_plane, st_row, st_pix, st_ch = planes_nhwc.stride()
+    if st_ch == 1 and st_row == planes_nhwc.shape[3] * st_pix and st_pix >= 32 and st_plane > 0 and st_img > 0:
+        return st_img, st_plane, st_pix
+    return None
+
+
 def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_warp, white_back=False, debug=False, impl=None,
                stratified=None, plane_index=None, out=None):
     """Fused ImportanceRenderer.forward. Returns (feat [B,R,C], depth [B,R,1], wsum [B,R,1][, debug dict]).
@@ -173,13 +185,10 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
         raise ValueError('planes batch and ray batch differ: pass plane_index')
     assert C == 32 and planes_nhwc.dtype == torch.float32
     impl = impl or render_impl
-    # a strided view is read in place by the tensor-core kernel as long as channels are contiguous and rows are W pixels
-    # apart (e.g. the backbone's NHWC [B,H,W,96] output viewed as [B,3,H,W,32]); everything else is made dense first
-    st_img, st_plane, st_row, st_pix, st_ch = planes_nhwc.stride()
-    strided = not planes_nhwc.is_contiguous()
-    if strided and not (st_ch == 1 and st_row == W * st_pix and st_pix >= 32 and st_plane > 0 and st_img > 0 and impl != 'simt'):
+    strides = None if impl == 'simt' else _in_place_strides(planes_nhwc)
+    if strides is None:
         planes_nhwc = planes_nhwc.contiguous()
-        strided = False
+    strided = strides is not None
     R = ray_origins.shape[1]
     o, d = _f32c(ray_origins), _f32c(ray_dirs)
     keep = []
@@ -247,7 +256,7 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
         a.out_depths_sorted = alloc('depths_sorted', (B, R, Sc + Sf), torch.float32).data_ptr()
     a.workspace = ws.data_ptr()
     if strided:
-        a.plane_strides[0], a.plane_strides[1], a.plane_strides[2] = st_img, st_plane, st_pix
+        a.plane_strides[0], a.plane_strides[1], a.plane_strides[2] = strides
     ev = None
     if kernel_events is not None:
         ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
@@ -345,13 +354,11 @@ def run_model(planes_nhwc, dec, coords, box_warp, impl=None, sigma_only=False):
     assert C == 32 and planes_nhwc.dtype == torch.float32
     impl = impl or render_impl
     use_tc = impl in ('auto', 'tc', 'tc_pairs') and dec.packed_tc is not None
-    strides = None
-    if not planes_nhwc.is_contiguous():
-        st_img, st_plane, st_row, st_pix, st_ch = planes_nhwc.stride()
-        if use_tc and st_ch == 1 and st_row == W * st_pix and st_pix >= 32 and st_plane > 0 and st_img > 0:
-            strides = (ctypes.c_int64 * 3)(st_img, st_plane, st_pix)       # read in place (see render_fwd)
-        else:
-            planes_nhwc = planes_nhwc.contiguous()
+    strides = _in_place_strides(planes_nhwc) if use_tc else None
+    if strides is None:
+        planes_nhwc = planes_nhwc.contiguous()
+    else:
+        strides = (ctypes.c_int64 * 3)(*strides)
     c = _f32c(coords)
     M = c.shape[1]
     dev = planes_nhwc.device
