@@ -304,15 +304,6 @@ int p3d_cross_entropy2d_bwd(const float* logits, const int64_t* target, const fl
                             const float* grad_loss, const float* sum_w, int N, int C, int64_t HW,
                             int64_t ignore_index, float* grad_logits, p3d_stream_t stream);
 
-/* Fused epilogue of an up=2 modulated conv (networks_stylegan2.py:324-331 + conv2d_resample.py:128):
- * y = clamp(lrelu(upfirdn2d(x, f, pad, gain=up^2) [* dcoef[n,c]] + noise[h,w]*noise_strength + b[c]) * act_gain).
- * One read of x, one write of y instead of three passes. Any of dcoef/noise/b may be NULL. */
-int p3d_fir_bias_act(const void* x, const float* f, const float* dcoef, const float* noise, const void* b, void* y,
-                     int dtype, const int32_t x_size[4], const int32_t y_size[4],
-                     int fw, int fh, int padx0, int pady0, float fir_gain,
-                     int act, float alpha, float act_gain, float clamp,
-                     int64_t noise_stride_n, p3d_stream_t stream);
-
 /* ---------------------------------------------------------------------------------------------
  * Tensor-core convolution path (training/networks_stylegan2.py:34-91 modulated_conv2d,
  * torch_utils/ops/conv2d_resample.py:48-143; the reference bottoms out in cuDNN through conv2d_gradfix.py:37-45)

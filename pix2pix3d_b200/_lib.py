@@ -10,13 +10,14 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libp3d.so')
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 _lib = None
 
-c_void_p, c_int, c_int32, c_int64, c_float, c_uint32 = (
-    ctypes.c_void_p, ctypes.c_int, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_uint32)
+c_void_p, c_int, c_int8, c_int32, c_int64, c_float, c_uint32 = (
+    ctypes.c_void_p, ctypes.c_int, ctypes.c_int8, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_uint32)
 
+P3D_UNSUPPORTED = -1
 P3D_F32, P3D_F16, P3D_F64 = 0, 1, 2
 DTYPE_CODE = {torch.float32: P3D_F32, torch.float16: P3D_F16, torch.float64: P3D_F64}
 
@@ -72,6 +73,51 @@ class FilteredLReluArgs(ctypes.Structure):  # p3d_filtered_lrelu_args_t
     ]
 
 
+class ConvArgs(ctypes.Structure):  # p3d_conv_args_t
+    _fields_ = [
+        ('x', c_void_p), ('w', c_void_p),
+        ('x_planes', c_int32), ('w_planes', c_int32), ('B', c_int32), ('Bw', c_int32),
+        ('H', c_int32), ('W', c_int32), ('C', c_int32), ('Cout', c_int32),
+        ('Cout_padded', c_int32), ('n_kblocks', c_int32), ('n_taps', c_int32),
+        ('tap_dy', c_int8 * 9), ('tap_dx', c_int8 * 9), ('tap_k', c_int8 * 9),
+        ('split', c_int32), ('gH', c_int32), ('gW', c_int32),
+        ('oH', c_int32), ('oW', c_int32), ('sy', c_int32), ('oy', c_int32),
+        ('sx', c_int32), ('ox', c_int32),
+        ('y', c_void_p), ('y_lo', c_void_p),
+        ('y_cstride', c_int32), ('y_coff', c_int32), ('out_mode', c_int32),
+        ('bias', c_void_p), ('noise', c_void_p), ('dscale', c_void_p),
+        ('act', c_int32), ('alpha', c_float), ('gain', c_float), ('clamp', c_float),
+        ('acc_scale', c_float),
+        ('up_prev', c_void_p), ('up_filter', c_void_p), ('round16', c_int32), ('out_nchw', c_int32),
+        ('stride', c_int32), ('launch_flags', c_int32), ('residual', c_void_p),
+        ('splitk_scratch', c_void_p), ('splitk_scratch_bytes', c_int64), ('noise_batch_stride', c_int64),
+        ('rgb_w', c_void_p), ('rgb_bias', c_void_p), ('rgb_prev', c_void_p), ('rgb_filter', c_void_p),
+        ('rgb_out', c_void_p), ('rgb_cout', c_int32), ('rgb_w_rows', c_int32), ('rgb_skip_x', c_int32),
+        ('rgb_clamp', c_float), ('rgb_acc_scale', c_float),
+    ]
+
+
+class WgradArgs(ctypes.Structure):  # p3d_wgrad_args_t
+    _fields_ = [
+        ('p', c_void_p), ('q', c_void_p),
+        ('B', c_int32), ('M', c_int32), ('N', c_int32), ('Lp', c_int32), ('Lq', c_int32),
+        ('q_phases', c_int32), ('n_taps', c_int32),
+        ('tap_phase', c_int32 * 9), ('tap_off', c_int32 * 9),
+        ('splits', c_int32),
+        ('scratch', c_void_p), ('scratch_bytes', c_int64),
+        ('p_scale', c_void_p), ('q_scale', c_void_p), ('dw', c_void_p),
+    ]
+
+
+class ModwDesc(ctypes.Structure):  # p3d_modw_desc_t
+    _fields_ = [
+        ('weight_t', c_void_p), ('wsq', c_void_p), ('styles_off', c_int64), ('out_off', c_int64),
+        ('Cout', c_int32), ('Cin', c_int32), ('ktaps', c_int32), ('Cout_padded', c_int32),
+        ('Cin_padded', c_int32), ('cin_offset', c_int32), ('demodulate', c_int32), ('planes', c_int32),
+        ('pre_scale', c_float), ('out_scale', c_float), ('first_block', c_int32), ('reserved', c_int32),
+    ]
+
+
 _SIGNATURES = {
     'p3d_abi_version': (c_int, []),
     'p3d_build_info': (ctypes.c_char_p, []),
@@ -110,9 +156,6 @@ _SIGNATURES = {
     'p3d_upfirdn2d': (c_int, [c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(c_int32), ctypes.POINTER(c_int64),
                               ctypes.POINTER(c_int32), ctypes.POINTER(c_int64), c_int, c_int, c_int, c_int, c_int, c_int,
                               c_int, c_int, c_int, c_float, c_void_p]),
-    'p3d_fir_bias_act': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                 ctypes.POINTER(c_int32), ctypes.POINTER(c_int32), c_int, c_int, c_int, c_int, c_float,
-                                 c_int, c_float, c_float, c_float, c_int64, c_void_p]),
     'p3d_decoder_mlp_fwd': (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),
     'p3d_decoder_mlp_bwd_workspace_floats': (c_int, []),
@@ -171,12 +214,6 @@ def lib():
     return _lib
 
 
-def check(status, what):
-    if status != 0:
-        msg = lib().p3d_status_string(status).decode()
-        raise RuntimeError(f'{what} failed: {msg} (status {status})')
-
-
 def stream_ptr(device=None):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -189,6 +226,25 @@ def ptr(t):
 launch_count = 0
 
 
-def bump(n=1):
+def launch(name, *args, device, launches=1, unsupported_ok=False):
+    """Call entry point `name` with `args` and the current stream of `device`, under that device's guard. A tensor argument
+    is passed as its data pointer (it must fill a c_void_p slot of _SIGNATURES: in an integer slot ctypes would truncate the
+    address), None as NULL. A non-zero status raises; on success `launches` (the kernels the call runs) is added to
+    launch_count. With `unsupported_ok`, P3D_UNSUPPORTED returns False instead of raising (the caller takes another path)."""
+    argtypes = _SIGNATURES[name][1]
+    cargs = list(args)
+    for i, a in enumerate(cargs):
+        if isinstance(a, torch.Tensor):
+            if argtypes[i] is not c_void_p:
+                raise TypeError(f'{name}: argument {i} is a tensor but p3d.h takes {argtypes[i].__name__} there')
+            cargs[i] = c_void_p(a.data_ptr())
+    with torch.cuda.device(device):
+        status = getattr(lib(), name)(*cargs, stream_ptr())
+    if status == P3D_UNSUPPORTED and unsupported_ok:
+        return False
+    if status != 0:
+        msg = lib().p3d_status_string(status).decode()
+        raise RuntimeError(f'{name} failed: {msg} (status {status})')
     global launch_count
-    launch_count += n
+    launch_count += launches
+    return True

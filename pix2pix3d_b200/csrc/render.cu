@@ -616,7 +616,7 @@ using namespace p3d;
 
 extern "C" {
 
-int p3d_abi_version(void) { return 8; }
+int p3d_abi_version(void) { return 9; }
 const char* p3d_build_info(void) { return "libp3d sm_90a " __DATE__ " " __TIME__; }
 const char* p3d_status_string(int status) {
     if (status == P3D_OK) return "ok";

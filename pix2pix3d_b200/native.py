@@ -17,11 +17,26 @@ TC_PACKED_BYTES = 65536 + 324 * 4
 # 'tc_pairs' (tensor-core decoder, ray-pair ownership: render_tc2.cu; sample counts <= 64)
 render_impl = 'auto'
 
-# when set to a list, render_fwd appends ('render_fwd', start_event, end_event) around its launch (bench.py)
+# when set to a list, timed_launch appends (tag, start_event, end_event, *extra) around its launch: render_fwd's
+# ('render_fwd', start, end) and the convolutions' (tag, start, end, flops, tensor_flops) (bench.py)
 kernel_events = None
 # when set to a dict, every render_fwd call also writes the kernel's bookkeeping (importance indices, fine depths, sort
 # permutation, interval weights) and leaves it there: lets tests score the bookkeeping of a whole G.synthesis call
 render_debug_sink = None
+
+
+def timed_launch(tag, name, *args, device, extra=(), unsupported_ok=False):
+    """_lib.launch, bracketed by CUDA events when kernel_events is set; a launch the library ran is appended there as
+    (tag, start, end, *extra)."""
+    if kernel_events is None:
+        return _lib.launch(name, *args, device=device, unsupported_ok=unsupported_ok)
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    ok = _lib.launch(name, *args, device=device, unsupported_ok=unsupported_ok)
+    end.record()
+    if ok:
+        kernel_events.append((tag, start, end, *extra))
+    return ok
 
 
 def _f32c(t):
@@ -39,11 +54,7 @@ def ray_sampler(cam2world, intrinsics, resolution):
     M = resolution * resolution
     origins = torch.empty(B, M, 3, device=c2w.device, dtype=torch.float32)
     dirs = torch.empty_like(origins)
-    with torch.cuda.device(c2w.device):
-        st = _lib.lib().p3d_ray_sampler(_lib.ptr(c2w), _lib.ptr(K), B, resolution, _lib.ptr(origins), _lib.ptr(dirs),
-                                        _lib.stream_ptr())
-    _lib.check(st, 'p3d_ray_sampler')
-    _lib.bump()
+    _lib.launch('p3d_ray_sampler', c2w, K, B, resolution, origins, dirs, device=c2w.device)
     return origins, dirs
 
 
@@ -54,10 +65,7 @@ def planes_to_channels_last(planes):
     C, H, W = shp[-3], shp[-2], shp[-1]
     N = p.numel() // (C * H * W)
     out = torch.empty(*shp[:-3], H, W, C, device=p.device, dtype=torch.float32)
-    with torch.cuda.device(p.device):
-        st = _lib.lib().p3d_planes_to_channels_last(_lib.ptr(p), _lib.ptr(out), N, C, H, W, _lib.stream_ptr())
-    _lib.check(st, 'p3d_planes_to_channels_last')
-    _lib.bump()
+    _lib.launch('p3d_planes_to_channels_last', p, out, N, C, H, W, device=p.device)
     return out
 
 
@@ -123,14 +131,9 @@ def pack_decoder(decoder):
         d.w2_gain[i], d.b2_gain[i] = float(fc2.weight_gain), float(fc2.bias_gain)
         d.sigmoid_mask[i] = masks[i]
     packed = torch.empty(PACKED_FLOATS, device=dev, dtype=torch.float32)
-    with torch.cuda.device(dev):
-        st = _lib.lib().p3d_pack_decoder(ctypes.byref(d), _lib.ptr(packed), _lib.stream_ptr())
-    _lib.check(st, 'p3d_pack_decoder')
+    _lib.launch('p3d_pack_decoder', ctypes.byref(d), packed, device=dev)
     packed_tc = torch.empty(TC_PACKED_BYTES, device=dev, dtype=torch.uint8)
-    with torch.cuda.device(dev):
-        st = _lib.lib().p3d_pack_decoder_tc(ctypes.byref(d), _lib.ptr(packed_tc), _lib.stream_ptr())
-    _lib.check(st, 'p3d_pack_decoder_tc')
-    _lib.bump(2)
+    _lib.launch('p3d_pack_decoder_tc', ctypes.byref(d), packed_tc, device=dev)
     del keep
     return PackedDecoder(packed, len(nets), sigma_net, masks, packed_tc)
 
@@ -142,10 +145,7 @@ def ray_limits_box(rays_o, rays_d, box_side_length):
     n = o.shape[0]
     tn = torch.empty(n, device=o.device, dtype=torch.float32)
     tf = torch.empty(n, device=o.device, dtype=torch.float32)
-    with torch.cuda.device(o.device):
-        st = _lib.lib().p3d_ray_limits_box(_lib.ptr(o), _lib.ptr(d), n, float(box_side_length), _lib.ptr(tn), _lib.ptr(tf), _lib.stream_ptr())
-    _lib.check(st, 'p3d_ray_limits_box')
-    _lib.bump()
+    _lib.launch('p3d_ray_limits_box', o, d, n, float(box_side_length), tn, tf, device=o.device)
     return tn.reshape(*lead, 1), tf.reshape(*lead, 1)
 
 
@@ -205,13 +205,9 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
     uu = None if u is None else _f32c(u)
     dev = planes_nhwc.device
     out = out or {}
-
-    def alloc(key, shape, dtype):
-        return _out_view(out[key], shape, dtype, dev) if key in out else torch.empty(*shape, device=dev, dtype=dtype)
-
-    feat = alloc('feat', (B, R, dec.out_channels), torch.float32)
-    depth = alloc('depth', (B, R, 1), torch.float32)
-    wsum = alloc('wsum', (B, R, 1), torch.float32)
+    feat = _alloc(out.get('feat'), (B, R, dec.out_channels), dev)
+    depth = _alloc(out.get('depth'), (B, R, 1), dev)
+    wsum = _alloc(out.get('wsum'), (B, R, 1), dev)
     ws = torch.empty(4, device=dev, dtype=torch.int32)
     a = _lib.RenderArgs()
     a.planes_nhwc, a.ray_origins, a.ray_dirs = planes_nhwc.data_ptr(), o.data_ptr(), d.data_ptr()
@@ -243,45 +239,33 @@ def render_fwd(planes_nhwc, dec, ray_origins, ray_dirs, depths_coarse, u, box_wa
     want_debug = debug or render_debug_sink is not None
     if want_debug:
         S = Sc + Sf
-        dbg['weights_final'] = alloc('weights_final', (B, R, S - 1), torch.float32)
-        dbg['perm'] = alloc('perm', (B, R, S), torch.int32)
+        dbg['weights_final'] = _alloc(out.get('weights_final'), (B, R, S - 1), dev)
+        dbg['perm'] = _alloc(out.get('perm'), (B, R, S), dev, torch.int32)
         a.dbg_weights_final, a.dbg_perm = dbg['weights_final'].data_ptr(), dbg['perm'].data_ptr()
         if Sf > 0:
-            dbg['weights_coarse'] = alloc('weights_coarse', (B, R, Sc - 1), torch.float32)
-            dbg['depths_fine'] = alloc('depths_fine', (B, R, Sf), torch.float32)
-            dbg['inds'] = alloc('inds', (B, R, Sf), torch.int32)
+            dbg['weights_coarse'] = _alloc(out.get('weights_coarse'), (B, R, Sc - 1), dev)
+            dbg['depths_fine'] = _alloc(out.get('depths_fine'), (B, R, Sf), dev)
+            dbg['inds'] = _alloc(out.get('inds'), (B, R, Sf), dev, torch.int32)
             a.dbg_weights_coarse = dbg['weights_coarse'].data_ptr()
             a.dbg_depths_fine, a.dbg_inds = dbg['depths_fine'].data_ptr(), dbg['inds'].data_ptr()
     if 'depths_sorted' in out:
-        a.out_depths_sorted = alloc('depths_sorted', (B, R, Sc + Sf), torch.float32).data_ptr()
+        a.out_depths_sorted = _alloc(out['depths_sorted'], (B, R, Sc + Sf), dev).data_ptr()
     a.workspace = ws.data_ptr()
     if strided:
         a.plane_strides[0], a.plane_strides[1], a.plane_strides[2] = strides
-    ev = None
-    if kernel_events is not None:
-        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-        ev[0].record()
     use_tc = impl in ('auto', 'tc', 'tc_pairs') and Sc % 8 == 0 and Sf % 8 == 0 and Sc <= 128 and Sf <= 128 and dec.packed_tc is not None
     if impl in ('tc', 'tc_pairs') and not use_tc:
         raise ValueError('tensor-core renderer needs sample counts that are multiples of 8')
     # ray-pair ownership fills its 64-row halves only at 64 samples per pass; at fewer samples per ray the row-tiled kernel
     # packs its tiles densely and the pair kernel would leave rows idle
     a.tc_variant = 1 if (impl == 'tc_pairs' or (impl == 'auto' and Sc == 64 and Sf == 64)) else 0
-    with torch.cuda.device(dev):
-        if use_tc:
-            a.decoder_packed = dec.packed_tc.data_ptr()
-            st = _lib.lib().p3d_render_fwd_tc(ctypes.byref(a), _lib.stream_ptr())
-        else:
-            if strided:   # the SIMT kernel reads dense planes only
-                dense = planes_nhwc.contiguous()
-                a.planes_nhwc = dense.data_ptr()
-                a.plane_strides[0] = a.plane_strides[1] = a.plane_strides[2] = 0
-            st = _lib.lib().p3d_render_fwd(ctypes.byref(a), _lib.stream_ptr())
-    if ev is not None:
-        ev[1].record()
-        kernel_events.append(('render_fwd', ev[0], ev[1]))
-    _lib.check(st, 'p3d_render_fwd')
-    _lib.bump()
+    if use_tc:
+        a.decoder_packed = dec.packed_tc.data_ptr()
+    elif strided:   # the SIMT kernel reads dense planes only
+        dense = planes_nhwc.contiguous()
+        a.planes_nhwc = dense.data_ptr()
+        a.plane_strides[0] = a.plane_strides[1] = a.plane_strides[2] = 0
+    timed_launch('render_fwd', 'p3d_render_fwd_tc' if use_tc else 'p3d_render_fwd', ctypes.byref(a), device=dev)
     if render_debug_sink is not None:
         render_debug_sink.update(dbg, feat=feat, depth=depth, wsum=wsum)
     if debug:
@@ -328,20 +312,17 @@ def render_bwd(planes_nhwc, params, sigma_net, masks, ray_origins, ray_dirs, dep
     out = out or {}
     g_planes = _alloc(out.get('planes'), (B, 3, H, W, 32), dev) if want_planes else None
     g_params = None
-    with torch.cuda.device(dev):
-        if want_params:
-            g_params = _alloc(out.get('params'), (n_nets, DECODER_PARAM_FLOATS), dev)
-            ws = out.get('workspace')
-            if ws is None:
-                ws = torch.empty(_lib.lib().p3d_render_bwd_workspace_floats(n_nets), device=dev, dtype=torch.float32)
-            else:
-                assert ws.dtype == torch.float32 and ws.device == dev and ws.is_contiguous(), 'out= buffer'
-            a.g_params, a.workspace, a.workspace_floats = g_params.data_ptr(), ws.data_ptr(), ws.numel()
-        if want_planes:
-            a.g_planes_nhwc = g_planes.data_ptr()
-        st = _lib.lib().p3d_render_bwd(ctypes.byref(a), _lib.stream_ptr())
-    _lib.check(st, 'p3d_render_bwd')
-    _lib.bump(1 + (n_nets if want_params else 0))
+    if want_params:
+        g_params = _alloc(out.get('params'), (n_nets, DECODER_PARAM_FLOATS), dev)
+        ws = out.get('workspace')
+        if ws is None:
+            ws = torch.empty(_lib.lib().p3d_render_bwd_workspace_floats(n_nets), device=dev, dtype=torch.float32)
+        else:
+            assert ws.dtype == torch.float32 and ws.device == dev and ws.is_contiguous(), 'out= buffer'
+        a.g_params, a.workspace, a.workspace_floats = g_params.data_ptr(), ws.data_ptr(), ws.numel()
+    if want_planes:
+        a.g_planes_nhwc = g_planes.data_ptr()
+    _lib.launch('p3d_render_bwd', ctypes.byref(a), device=dev, launches=1 + (n_nets if want_params else 0))
     return g_planes, g_params
 
 
@@ -366,18 +347,12 @@ def run_model(planes_nhwc, dec, coords, box_warp, impl=None, sigma_only=False):
     rgb = None if sigma_only else torch.empty(B, M, dec.out_channels, device=dev, dtype=torch.float32)
     sigma = torch.empty(B, M, 1, device=dev, dtype=torch.float32)
     masks = (ctypes.c_uint32 * 2)(dec.masks[0], dec.masks[1])
-    with torch.cuda.device(dev):
-        if use_tc:
-            st = _lib.lib().p3d_run_model_tc(_lib.ptr(planes_nhwc), strides, _lib.ptr(c), _lib.ptr(dec.packed_tc), dec.n_nets,
-                                             dec.sigma_net, masks, B, M, H, W, 2.0 / float(box_warp), _lib.ptr(rgb),
-                                             _lib.ptr(sigma), _lib.stream_ptr())
-            _lib.check(st, 'p3d_run_model_tc')
-        else:
-            st = _lib.lib().p3d_run_model(_lib.ptr(planes_nhwc), _lib.ptr(c), _lib.ptr(dec.packed), dec.n_nets, dec.sigma_net,
-                                          masks, B, M, H, W, 2.0 / float(box_warp), _lib.ptr(rgb), _lib.ptr(sigma),
-                                          _lib.stream_ptr())
-            _lib.check(st, 'p3d_run_model')
-    _lib.bump()
+    if use_tc:
+        _lib.launch('p3d_run_model_tc', planes_nhwc, strides, c, dec.packed_tc, dec.n_nets, dec.sigma_net, masks, B, M, H, W,
+                    2.0 / float(box_warp), rgb, sigma, device=dev)
+    else:
+        _lib.launch('p3d_run_model', planes_nhwc, c, dec.packed, dec.n_nets, dec.sigma_net, masks, B, M, H, W,
+                    2.0 / float(box_warp), rgb, sigma, device=dev)
     return rgb, sigma
 
 
@@ -393,11 +368,7 @@ def sample_from_planes(planes_nhwc, coords, box_warp, out=None):
     c = _f32c(coords)
     M = c.shape[1]
     out = _alloc(out, (B, 3, M, 32), planes_nhwc.device)
-    with torch.cuda.device(planes_nhwc.device):
-        st = _lib.lib().p3d_sample_from_planes(_lib.ptr(planes_nhwc), _lib.ptr(c), B, M, H, W, 2.0 / float(box_warp),
-                                               _lib.ptr(out), _lib.stream_ptr())
-    _lib.check(st, 'p3d_sample_from_planes')
-    _lib.bump()
+    _lib.launch('p3d_sample_from_planes', planes_nhwc, c, B, M, H, W, 2.0 / float(box_warp), out, device=planes_nhwc.device)
     return out
 
 
@@ -412,11 +383,7 @@ def ray_march(colors, densities, depths, white_back=False, out=None):
     depth = _alloc(out.get('depth'), (B, R, 1), dev)
     weights = _alloc(out.get('weights'), (B, R, S - 1, 1), dev)
     ws = torch.empty(4, device=dev, dtype=torch.int32)
-    with torch.cuda.device(dev):
-        st = _lib.lib().p3d_ray_march(_lib.ptr(col), _lib.ptr(den), _lib.ptr(dep), B * R, S, Cc, 1 if white_back else 0,
-                                      _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(weights), _lib.ptr(ws), _lib.stream_ptr())
-    _lib.check(st, 'p3d_ray_march')
-    _lib.bump()
+    _lib.launch('p3d_ray_march', col, den, dep, B * R, S, Cc, 1 if white_back else 0, rgb, depth, weights, ws, device=dev)
     return rgb, depth, weights
 
 
@@ -426,11 +393,7 @@ def sample_from_planes_bwd(grad_features, coords, box_warp, H, W, out=None):
     c = _f32c(coords)
     B, _, M, _ = g.shape
     out = _alloc(out, (B, 3, H, W, 32), g.device)
-    with torch.cuda.device(g.device):
-        st = _lib.lib().p3d_sample_from_planes_bwd(_lib.ptr(g), _lib.ptr(c), B, M, H, W, 2.0 / float(box_warp), _lib.ptr(out),
-                                                   _lib.stream_ptr())
-    _lib.check(st, 'p3d_sample_from_planes_bwd')
-    _lib.bump()
+    _lib.launch('p3d_sample_from_planes_bwd', g, c, B, M, H, W, 2.0 / float(box_warp), out, device=g.device)
     return out
 
 
@@ -446,12 +409,8 @@ def ray_march_bwd(colors, densities, depths, g_rgb, g_depth, g_weights, depth_ra
     out = out or {}
     g_col = _alloc(out.get('colors'), tuple(col.shape), col.device)
     g_den = _alloc(out.get('densities'), tuple(den.shape), col.device)
-    with torch.cuda.device(col.device):
-        st = _lib.lib().p3d_ray_march_bwd(_lib.ptr(col), _lib.ptr(den), _lib.ptr(dep), _lib.ptr(grgb), _lib.ptr(gdep),
-                                          _lib.ptr(gw), _lib.ptr(rng), B * R, S, Cc, 1 if white_back else 0, _lib.ptr(g_col),
-                                          _lib.ptr(g_den), _lib.stream_ptr())
-    _lib.check(st, 'p3d_ray_march_bwd')
-    _lib.bump()
+    _lib.launch('p3d_ray_march_bwd', col, den, dep, grgb, gdep, gw, rng, B * R, S, Cc, 1 if white_back else 0, g_col, g_den,
+                device=col.device)
     return g_col, g_den
 
 
@@ -464,11 +423,7 @@ def sample_importance(z_vals, weights, u, return_inds=False, out=None):
     bufs = out or {}
     out = _alloc(bufs.get('samples'), (N, Sf), z.device)
     inds = _alloc(bufs.get('inds'), (N, Sf), z.device, torch.int32) if return_inds else None
-    with torch.cuda.device(z.device):
-        st = _lib.lib().p3d_sample_importance(_lib.ptr(z), _lib.ptr(w), _lib.ptr(uu), N, S, Sf, _lib.ptr(out),
-                                              _lib.ptr(inds), _lib.stream_ptr())
-    _lib.check(st, 'p3d_sample_importance')
-    _lib.bump()
+    _lib.launch('p3d_sample_importance', z, w, uu, N, S, Sf, out, inds, device=z.device)
     return (out, inds) if return_inds else out
 
 
@@ -490,12 +445,8 @@ def decoder_mlp_fwd(feats, w1, b1, w2, b2, mask, want_saved=False, out=None):
         r['pre'] = _alloc(out.get('pre'), (n * m, 64), f.device)
         if mask:
             r['sig'] = _alloc(out.get('sig'), (n * m, 32), f.device)
-    with torch.cuda.device(f.device):
-        st = _lib.lib().p3d_decoder_mlp_fwd(_lib.ptr(f), n, m, _lib.ptr(w1c), _lib.ptr(b1c), _lib.ptr(w2c), _lib.ptr(b2c), int(mask),
-                                            _lib.ptr(r['rgb']), _lib.ptr(r['sigma']), _lib.ptr(r.get('pre')), _lib.ptr(r.get('sig')),
-                                            _lib.stream_ptr())
-    _lib.check(st, 'p3d_decoder_mlp_fwd')
-    _lib.bump()
+    _lib.launch('p3d_decoder_mlp_fwd', f, n, m, w1c, b1c, w2c, b2c, int(mask), r['rgb'], r['sigma'], r.get('pre'), r.get('sig'),
+                device=f.device)
     return r
 
 
@@ -510,14 +461,10 @@ def decoder_mlp_bwd(feats, w1, b1, w2, b2, mask, pre, sig, g_rgb, g_sigma, out=N
     out = out or {}
     g_feats = _alloc(out.get('feats'), tuple(f.shape), f.device)
     g_params = _alloc(out.get('params'), (DECODER_PARAM_FLOATS,), f.device)
-    with torch.cuda.device(f.device):
-        nws = _lib.lib().p3d_decoder_mlp_bwd_workspace_floats()
-        ws = torch.empty(nws, device=f.device, dtype=torch.float32)
-        st = _lib.lib().p3d_decoder_mlp_bwd(_lib.ptr(f), _lib.ptr(pre), _lib.ptr(sig), n, m, _lib.ptr(w1c), _lib.ptr(b1c), _lib.ptr(w2c),
-                                            _lib.ptr(b2c), int(mask), _lib.ptr(gr), _lib.ptr(gs), _lib.ptr(g_feats), _lib.ptr(g_params),
-                                            _lib.ptr(ws), nws, _lib.stream_ptr())
-    _lib.check(st, 'p3d_decoder_mlp_bwd')
-    _lib.bump(2)
+    nws = _lib.lib().p3d_decoder_mlp_bwd_workspace_floats()
+    ws = torch.empty(nws, device=f.device, dtype=torch.float32)
+    _lib.launch('p3d_decoder_mlp_bwd', f, pre, sig, n, m, w1c, b1c, w2c, b2c, int(mask), gr, gs, g_feats, g_params, ws, nws,
+                device=f.device, launches=2)
     return dict(feats=g_feats, params=g_params)
 
 
@@ -584,9 +531,6 @@ def fc_bias_act(x, weight, bias, weight_gain, bias_gain, act, alpha, act_gain):
     xc, wc = _f32c(x.detach()), _f32c(weight.detach())
     bc = None if bias is None else _f32c(bias.detach())
     y = torch.empty(xc.shape[0], wc.shape[0], device=xc.device, dtype=torch.float32)
-    with torch.cuda.device(xc.device):
-        st = _lib.lib().p3d_fc_bias_act(_lib.ptr(xc), _lib.ptr(wc), _lib.ptr(bc), _lib.ptr(y), xc.shape[0], xc.shape[1], wc.shape[0],
-                                        float(weight_gain), float(bias_gain), int(act), float(alpha), float(act_gain), _lib.stream_ptr())
-    _lib.check(st, 'p3d_fc_bias_act')
-    _lib.bump()
+    _lib.launch('p3d_fc_bias_act', xc, wc, bc, y, xc.shape[0], xc.shape[1], wc.shape[0], float(weight_gain), float(bias_gain),
+                int(act), float(alpha), float(act_gain), device=xc.device)
     return y

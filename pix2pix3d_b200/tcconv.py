@@ -7,35 +7,9 @@ import os
 
 import torch
 
-from . import _lib
-
-c_int8 = ctypes.c_int8
+from . import _lib, native
 
 WEIGHT_SCALE = 128.0   # power of two folded into the fp16 weights so that the `lo` halves stay normal numbers
-
-
-class ConvArgs(ctypes.Structure):  # p3d_conv_args_t
-    _fields_ = [
-        ('x', ctypes.c_void_p), ('w', ctypes.c_void_p),
-        ('x_planes', ctypes.c_int32), ('w_planes', ctypes.c_int32), ('B', ctypes.c_int32), ('Bw', ctypes.c_int32),
-        ('H', ctypes.c_int32), ('W', ctypes.c_int32), ('C', ctypes.c_int32), ('Cout', ctypes.c_int32),
-        ('Cout_padded', ctypes.c_int32), ('n_kblocks', ctypes.c_int32), ('n_taps', ctypes.c_int32),
-        ('tap_dy', c_int8 * 9), ('tap_dx', c_int8 * 9), ('tap_k', c_int8 * 9),
-        ('split', ctypes.c_int32), ('gH', ctypes.c_int32), ('gW', ctypes.c_int32),
-        ('oH', ctypes.c_int32), ('oW', ctypes.c_int32), ('sy', ctypes.c_int32), ('oy', ctypes.c_int32),
-        ('sx', ctypes.c_int32), ('ox', ctypes.c_int32),
-        ('y', ctypes.c_void_p), ('y_lo', ctypes.c_void_p),
-        ('y_cstride', ctypes.c_int32), ('y_coff', ctypes.c_int32), ('out_mode', ctypes.c_int32),
-        ('bias', ctypes.c_void_p), ('noise', ctypes.c_void_p), ('dscale', ctypes.c_void_p),
-        ('act', ctypes.c_int32), ('alpha', ctypes.c_float), ('gain', ctypes.c_float), ('clamp', ctypes.c_float),
-        ('acc_scale', ctypes.c_float),
-        ('up_prev', ctypes.c_void_p), ('up_filter', ctypes.c_void_p), ('round16', ctypes.c_int32), ('out_nchw', ctypes.c_int32),
-        ('stride', ctypes.c_int32), ('launch_flags', ctypes.c_int32), ('residual', ctypes.c_void_p),
-        ('splitk_scratch', ctypes.c_void_p), ('splitk_scratch_bytes', ctypes.c_int64), ('noise_batch_stride', ctypes.c_int64),
-        ('rgb_w', ctypes.c_void_p), ('rgb_bias', ctypes.c_void_p), ('rgb_prev', ctypes.c_void_p), ('rgb_filter', ctypes.c_void_p),
-        ('rgb_out', ctypes.c_void_p), ('rgb_cout', ctypes.c_int32), ('rgb_w_rows', ctypes.c_int32), ('rgb_skip_x', ctypes.c_int32),
-        ('rgb_clamp', ctypes.c_float), ('rgb_acc_scale', ctypes.c_float),
-    ]
 
 
 def pad_to(n, m):
@@ -57,11 +31,7 @@ def to_nhwc_f16(x, c_padded=None, planes=1, out=None):
     n, c, h, w = x.shape
     cp = c_padded or c
     out = _out(out, (planes, n, h, w, cp), x, torch.float16)
-    with torch.cuda.device(x.device):
-        st = _lib.lib().p3d_nchw_to_nhwc_f16(_lib.ptr(x), _lib.DTYPE_CODE[x.dtype], n, c, h, w, cp, planes, _lib.ptr(out),
-                                             _lib.stream_ptr())
-    _lib.check(st, 'p3d_nchw_to_nhwc_f16')
-    _lib.bump()
+    _lib.launch('p3d_nchw_to_nhwc_f16', x, _lib.DTYPE_CODE[x.dtype], n, c, h, w, cp, planes, out, device=x.device)
     return out
 
 
@@ -71,10 +41,7 @@ def nhwc_to_nchw_f32(x, channels=None, c_offset=0, out=None):
     n, h, w, cs = x.shape
     c = channels or cs
     out = _out(out, (n, c, h, w), x, torch.float32)
-    with torch.cuda.device(x.device):
-        st = _lib.lib().p3d_nhwc_to_nchw_f32(_lib.ptr(x), n, c, h, w, cs, c_offset, _lib.ptr(out), _lib.stream_ptr())
-    _lib.check(st, 'p3d_nhwc_to_nchw_f32')
-    _lib.bump()
+    _lib.launch('p3d_nhwc_to_nchw_f32', x, n, c, h, w, cs, c_offset, out, device=x.device)
     return out
 
 
@@ -84,10 +51,7 @@ def prepare_weights(weight):
     o, i, kh, kw = w.shape
     wt = torch.empty(o, kh * kw, i, device=w.device, dtype=torch.float32)
     wsq = torch.empty(o, i, device=w.device, dtype=torch.float32)
-    with torch.cuda.device(w.device):
-        st = _lib.lib().p3d_prepare_weights(_lib.ptr(w), o, i, kh * kw, _lib.ptr(wt), _lib.ptr(wsq), _lib.stream_ptr())
-    _lib.check(st, 'p3d_prepare_weights')
-    _lib.bump()
+    _lib.launch('p3d_prepare_weights', w, o, i, kh * kw, wt, wsq, device=w.device)
     return wt, wsq
 
 
@@ -103,38 +67,19 @@ def modulate_weights(weight, styles, demodulate=True, pre_scale=1.0, planes=1, c
     nchunk = ip // 8
     if prepared is not None and ip % 8 == 0 and nchunk <= 256 and 256 % nchunk == 0:
         wt, wsq = prepared
-        with torch.cuda.device(s.device):
-            st = _lib.lib().p3d_modulate_weights_t(_lib.ptr(wt), _lib.ptr(wsq), _lib.ptr(s), b, o, i, kh * kw, op, ip, cin_offset,
-                                                   1 if demodulate else 0, float(pre_scale), float(out_scale), planes, _lib.ptr(out),
-                                                   _lib.stream_ptr())
-        _lib.check(st, 'p3d_modulate_weights_t')
-        _lib.bump()
+        _lib.launch('p3d_modulate_weights_t', wt, wsq, s, b, o, i, kh * kw, op, ip, cin_offset, 1 if demodulate else 0,
+                    float(pre_scale), float(out_scale), planes, out, device=s.device)
         return out
     w = weight.detach().float().contiguous()
-    with torch.cuda.device(w.device):
-        st = _lib.lib().p3d_modulate_weights(_lib.ptr(w), _lib.ptr(s), b, o, i, kh * kw, op, ip, cin_offset, 1 if demodulate else 0,
-                                             float(pre_scale), float(out_scale), planes, _lib.ptr(out), _lib.stream_ptr())
-    _lib.check(st, 'p3d_modulate_weights')
-    _lib.bump()
+    _lib.launch('p3d_modulate_weights', w, s, b, o, i, kh * kw, op, ip, cin_offset, 1 if demodulate else 0, float(pre_scale),
+                float(out_scale), planes, out, device=w.device)
     return out
-
-
-class ModwDesc(ctypes.Structure):  # p3d_modw_desc_t
-    _fields_ = [
-        ('weight_t', ctypes.c_void_p), ('wsq', ctypes.c_void_p), ('styles_off', ctypes.c_int64), ('out_off', ctypes.c_int64),
-        ('Cout', ctypes.c_int32), ('Cin', ctypes.c_int32), ('ktaps', ctypes.c_int32), ('Cout_padded', ctypes.c_int32),
-        ('Cin_padded', ctypes.c_int32), ('cin_offset', ctypes.c_int32), ('demodulate', ctypes.c_int32), ('planes', ctypes.c_int32),
-        ('pre_scale', ctypes.c_float), ('out_scale', ctypes.c_float), ('first_block', ctypes.c_int32), ('reserved', ctypes.c_int32),
-    ]
 
 
 def modulate_weights_batch(descs_dev, block_layer_dev, n_blocks, styles_flat, out_flat, batch):
     """One launch for every layer described by `descs_dev` (device bytes of ModwDesc[]); see p3d_modulate_weights_batch."""
-    with torch.cuda.device(styles_flat.device):
-        st = _lib.lib().p3d_modulate_weights_batch(_lib.ptr(descs_dev), _lib.ptr(block_layer_dev), n_blocks, _lib.ptr(styles_flat),
-                                                   _lib.ptr(out_flat), batch, _lib.stream_ptr())
-    _lib.check(st, 'p3d_modulate_weights_batch')
-    _lib.bump()
+    _lib.launch('p3d_modulate_weights_batch', descs_dev, block_layer_dev, n_blocks, styles_flat, out_flat, batch,
+                device=styles_flat.device)
 
 
 def affine_batch(ws, weight, bias, meta, out_numel, out=None):
@@ -143,11 +88,7 @@ def affine_batch(ws, weight, bias, meta, out_numel, out=None):
     ws = ws.detach().float().contiguous()
     b, num_ws, w_dim = ws.shape
     out = _out(out, (out_numel,), ws, torch.float32)
-    with torch.cuda.device(ws.device):
-        st = _lib.lib().p3d_affine_batch(_lib.ptr(ws), _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(meta), _lib.ptr(out), b, num_ws, w_dim,
-                                         weight.shape[0], _lib.stream_ptr())
-    _lib.check(st, 'p3d_affine_batch')
-    _lib.bump()
+    _lib.launch('p3d_affine_batch', ws, weight, bias, meta, out, b, num_ws, w_dim, weight.shape[0], device=ws.device)
     return out
 
 
@@ -173,7 +114,7 @@ def _conv_args(x, w, cout, taps, grid_hw, out, out_lo=None, out_mode=0, out_map=
     wp, bw, op, kk = w.shape
     assert x.dtype == torch.float16 and w.dtype == torch.float16 and x.is_contiguous() and w.is_contiguous()
     assert kk % c == 0
-    a = ConvArgs()
+    a = _lib.ConvArgs()
     a.x, a.w = x.data_ptr(), w.data_ptr()
     a.x_planes, a.w_planes, a.B, a.Bw, a.H, a.W, a.C = xp, wp, b, bw, h, wd, c
     a.Cout, a.Cout_padded, a.n_kblocks, a.n_taps = cout, op, kk // c, len(taps)
@@ -226,54 +167,32 @@ def _conv_args(x, w, cout, taps, grid_hw, out, out_lo=None, out_mode=0, out_map=
     return a
 
 
-def _launch(device, call, name, flops, split, tag='conv_gemm'):
-    """Run one libp3d convolution launch; with native.kernel_events set, bracket it with CUDA events (bench.py's tensor roofline
-    counts the 'conv_gemm' ones)."""
-    from . import native
-    ev = None
-    if native.kernel_events is not None:
-        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-        ev[0].record()
-    with torch.cuda.device(device):
-        st = call()
-    if ev is not None:
-        ev[1].record()
-        # algorithmic FLOPs of the convolution this launch implements (one pass); the fp32 layers execute 3x that on the
-        # tensor pipe (hi*hi + hi*lo + lo*hi)
-        native.kernel_events.append((tag, ev[0], ev[1], flops, flops * (3 if split else 1)))
-    _lib.check(st, name)
-    _lib.bump()
+def _launch(tag, flops, split, name, *args, device, unsupported_ok=False):
+    """One libp3d convolution launch, timed under `tag` when native.kernel_events is set (bench.py's tensor roofline counts the
+    'conv_gemm' ones). `flops`: algorithmic FLOPs of what the launch implements (one pass); the fp32 layers execute 3x that on
+    the tensor pipe (hi*hi + hi*lo + lo*hi)."""
+    return native.timed_launch(tag, name, *args, device=device, extra=(flops, flops * (3 if split else 1)),
+                               unsupported_ok=unsupported_ok)
+
+
+def _conv_gemm(x, w, cout, taps, grid_hw, out, split, unsupported_ok, kw):
+    a = _conv_args(x, w, cout, taps, grid_hw, out, split=split, **kw)
+    # the fused ToRGB (rgb=) adds rgb_cout dot products of length cout per output pixel
+    flops = 2.0 * x.shape[1] * grid_hw[0] * grid_hw[1] * cout * (len(taps) * x.shape[4] + (a.rgb_cout if a.rgb_w else 0))
+    return _launch('conv_gemm', flops, split, 'p3d_conv_gemm', ctypes.byref(a), device=x.device, unsupported_ok=unsupported_ok)
 
 
 def conv_gemm(x, w, cout, taps, grid_hw, out, split=False, **kw):
     """x [xp,B,H,W,C] fp16, w [wp,Bw,Op,nk*C] fp16; taps: list of (dy, dx, kblock); grid_hw: computed grid;
     out: NHWC tensor [B,oH,oW,Cs] (fp16 or fp32); out_map = (sy, oy, sx, ox)."""
-    a = _conv_args(x, w, cout, taps, grid_hw, out, split=split, **kw)
-    flops = 2.0 * x.shape[1] * grid_hw[0] * grid_hw[1] * cout * len(taps) * x.shape[4]
-    _launch(x.device, lambda: _lib.lib().p3d_conv_gemm(ctypes.byref(a), _lib.stream_ptr()), 'p3d_conv_gemm', flops, split)
+    _conv_gemm(x, w, cout, taps, grid_hw, out, split, False, kw)
     return out
 
 
 def conv_gemm_try(x, w, cout, taps, grid_hw, out, split=False, **kw):
     """conv_gemm that reports P3D_UNSUPPORTED (-1) as False instead of raising: for optional fusions (`rgb=`) whose launch shape
     the library decides on; the caller then takes the unfused sequence."""
-    from . import native
-    a = _conv_args(x, w, cout, taps, grid_hw, out, split=split, **kw)
-    ev = None
-    if native.kernel_events is not None:
-        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-        ev[0].record()
-    with torch.cuda.device(x.device):
-        st = _lib.lib().p3d_conv_gemm(ctypes.byref(a), _lib.stream_ptr())
-    if st == -1:
-        return False
-    if ev is not None:
-        ev[1].record()
-        flops = 2.0 * x.shape[1] * grid_hw[0] * grid_hw[1] * cout * (len(taps) * x.shape[4] + (a.rgb_cout if a.rgb_w else 0))
-        native.kernel_events.append(('conv_gemm', ev[0], ev[1], flops, flops * (3 if split else 1)))
-    _lib.check(st, 'p3d_conv_gemm')
-    _lib.bump()
-    return True
+    return _conv_gemm(x, w, cout, taps, grid_hw, out, split, True, kw)
 
 
 TAPS_3X3 = [(ky - 1, kx - 1, ky * 3 + kx) for ky in range(3) for kx in range(3)]
@@ -302,13 +221,13 @@ def conv_transpose3x3_s2(x, w, cout, out, split=False, acc_scale=1.0 / WEIGHT_SC
             conv_gemm(x, w, cout, tconv_phase_taps(py, px), ghw, out, out_mode=mode, out_map=(2, py, 2, px), split=split,
                       acc_scale=acc_scale)
         return out
-    arr = (ConvArgs * 4)()
+    arr = (_lib.ConvArgs * 4)()
     flops = 0.0
     for k, (py, px, ghw) in enumerate(phases):
         taps = tconv_phase_taps(py, px)
         arr[k] = _conv_args(x, w, cout, taps, ghw, out, out_mode=mode, out_map=(2, py, 2, px), split=split, acc_scale=acc_scale)
         flops += 2.0 * b * ghw[0] * ghw[1] * cout * len(taps) * c
-    _launch(x.device, lambda: _lib.lib().p3d_conv_gemm_phases(arr, 4, _lib.stream_ptr()), 'p3d_conv_gemm_phases', flops, split)
+    _launch('conv_gemm', flops, split, 'p3d_conv_gemm_phases', arr, 4, device=x.device)
     return out
 
 
@@ -350,21 +269,13 @@ def fir_act_nhwc(x, f, noise, bias, out_planes, out_hw, pad0=(1, 1), fir_gain=4.
     if noise is not None:
         assert noise.is_contiguous() and noise.dtype == torch.float32 and noise.shape[-2:] == (oh, ow)
     sep = separable_factors(f) if (FIR_VARIANT == 3 and not split_in) else None
-    with torch.cuda.device(x.device):
-        if sep is not None:
-            st = _lib.lib().p3d_fir_act_nhwc_sep(_lib.ptr(x), _lib.DTYPE_CODE[x.dtype], sep[0], sep[1], _lib.ptr(noise), _lib.ptr(bias),
-                                                 _lib.ptr(y), out_planes, b, ih, iw, oh, ow, c, pad0[0], pad0[1], fir_gain, act, alpha,
-                                                 act_gain, clamp, nbs, _lib.stream_ptr())
-        elif split_in:
-            st = _lib.lib().p3d_fir_act_nhwc_split(_lib.ptr(x), _lib.ptr(f), _lib.ptr(noise), _lib.ptr(bias), _lib.ptr(y), out_planes, b,
-                                                   ih, iw, oh, ow, c, pad0[0], pad0[1], fir_gain, act, alpha, act_gain, clamp,
-                                                   nbs, _lib.stream_ptr())
-        else:
-            st = _lib.lib().p3d_fir_act_nhwc(_lib.ptr(x), _lib.DTYPE_CODE[x.dtype], _lib.ptr(f), _lib.ptr(noise), _lib.ptr(bias),
-                                             _lib.ptr(y), out_planes, b, ih, iw, oh, ow, c, pad0[0], pad0[1], fir_gain, act, alpha,
-                                             act_gain, clamp, nbs, _lib.stream_ptr())
-    _lib.check(st, 'p3d_fir_act_nhwc')
-    _lib.bump()
+    tail = (out_planes, b, ih, iw, oh, ow, c, pad0[0], pad0[1], fir_gain, act, alpha, act_gain, clamp, nbs)
+    if sep is not None:
+        _lib.launch('p3d_fir_act_nhwc_sep', x, _lib.DTYPE_CODE[x.dtype], sep[0], sep[1], noise, bias, y, *tail, device=x.device)
+    elif split_in:
+        _lib.launch('p3d_fir_act_nhwc_split', x, f, noise, bias, y, *tail, device=x.device)
+    else:
+        _lib.launch('p3d_fir_act_nhwc', x, _lib.DTYPE_CODE[x.dtype], f, noise, bias, y, *tail, device=x.device)
     return y
 
 
@@ -372,28 +283,13 @@ def upsample2x_nhwc(x, f, out=None):
     """upfirdn2d.upsample2d(x, f) on fp32 NHWC [B,H,W,C] -> [B,2H,2W,C] (into `out` when given)."""
     b, h, w, c = x.shape
     y = _out(out, (b, 2 * h, 2 * w, c), x, torch.float32)
-    with torch.cuda.device(x.device):
-        st = _lib.lib().p3d_upsample2x_nhwc(_lib.ptr(x), _lib.ptr(f), _lib.ptr(y), b, h, w, c, _lib.stream_ptr())
-    _lib.check(st, 'p3d_upsample2x_nhwc')
-    _lib.bump()
+    _lib.launch('p3d_upsample2x_nhwc', x, f, y, b, h, w, c, device=x.device)
     return y
 
 
 # ----------------------------------------------------------------------------------------------
 # weight gradients (p3d_conv_wgrad)
 # ----------------------------------------------------------------------------------------------
-class WgradArgs(ctypes.Structure):  # p3d_wgrad_args_t
-    _fields_ = [
-        ('p', ctypes.c_void_p), ('q', ctypes.c_void_p),
-        ('B', ctypes.c_int32), ('M', ctypes.c_int32), ('N', ctypes.c_int32), ('Lp', ctypes.c_int32), ('Lq', ctypes.c_int32),
-        ('q_phases', ctypes.c_int32), ('n_taps', ctypes.c_int32),
-        ('tap_phase', ctypes.c_int32 * 9), ('tap_off', ctypes.c_int32 * 9),
-        ('splits', ctypes.c_int32),
-        ('scratch', ctypes.c_void_p), ('scratch_bytes', ctypes.c_int64),
-        ('p_scale', ctypes.c_void_p), ('q_scale', ctypes.c_void_p), ('dw', ctypes.c_void_p),
-    ]
-
-
 WGRAD_BM, WGRAD_BK = 128, 64       # P channels per tile, pixels per k-step (conv_wgrad.cu)
 WGRAD_MAX_SPLITS = 64
 
@@ -458,11 +354,7 @@ def wgrad_operand(x, grid_h, wp, stride, phases, top, scale):
     assert x.is_cuda and x.dtype == torch.float32 and x.ndim == 4
     b, c, h, w = x.shape
     out = torch.empty(2, b, phases, c, grid_h * wp, device=x.device, dtype=torch.float16)
-    with torch.cuda.device(x.device):
-        st = _lib.lib().p3d_wgrad_operand(_lib.ptr(x), b, c, h, w, stride, phases, grid_h, wp, top, _lib.ptr(scale), _lib.ptr(out),
-                                          _lib.stream_ptr())
-    _lib.check(st, 'p3d_wgrad_operand')
-    _lib.bump()
+    _lib.launch('p3d_wgrad_operand', x, b, c, h, w, stride, phases, grid_h, wp, top, scale, out, device=x.device)
     return out
 
 
@@ -485,7 +377,7 @@ def conv_wgrad(p, q, k, stride, p_scale=None, q_scale=None, splits=None):
     qh = wgrad_operand(q, plan['hq'], plan['wp'], stride, plan['q_phases'], plan['q_top'], q_scale)
     scratch = torch.empty(plan['scratch_floats'], device=p.device, dtype=torch.float32)
     dw = torch.empty(m, n, k, k, device=p.device, dtype=torch.float32)
-    a = WgradArgs()
+    a = _lib.WgradArgs()
     a.p, a.q = ph.data_ptr(), qh.data_ptr()
     a.B, a.M, a.N, a.Lp, a.Lq, a.q_phases, a.n_taps = b, m, n, plan['Lp'], plan['Lq'], plan['q_phases'], len(plan['taps'])
     for t, (phase, off) in enumerate(plan['taps']):
@@ -494,6 +386,5 @@ def conv_wgrad(p, q, k, stride, p_scale=None, q_scale=None, splits=None):
     a.scratch, a.scratch_bytes = scratch.data_ptr(), scratch.numel() * 4
     a.p_scale, a.q_scale, a.dw = p_scale.data_ptr(), q_scale.data_ptr(), dw.data_ptr()
     flops = 2.0 * b * h * w * m * n * k * k
-    _launch(p.device, lambda: _lib.lib().p3d_conv_wgrad(ctypes.byref(a), _lib.stream_ptr()), 'p3d_conv_wgrad', flops, True,
-            tag='conv_wgrad')
+    _launch('conv_wgrad', flops, True, 'p3d_conv_wgrad', ctypes.byref(a), device=p.device)
     return dw

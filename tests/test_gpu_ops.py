@@ -150,30 +150,6 @@ def test_upfirdn2d_hot_shapes_and_gradient():
     assert torch.autograd.gradgradcheck(lambda a: upfirdn2d.upfirdn2d(a, f64, padding=[1, 1, 1, 1]), (x,))
 
 
-def test_fused_fir_bias_act_equals_composition():
-    """p3d_fir_bias_act = upfirdn2d -> (*dcoef) + noise -> bias_act, the epilogue of an up=2 SynthesisLayer."""
-    import ctypes
-    from pix2pix3d_b200 import _lib
-    from pix2pix3d_b200.torch_utils.ops import bias_act, upfirdn2d
-    torch.manual_seed(1)
-    f = upfirdn2d.setup_filter([1, 3, 3, 1]).cuda()
-    for dtype, tol in ((torch.float32, 2e-6), (torch.float16, 2e-3)):
-        x = torch.randn(2, 6, 17, 17, device='cuda').to(dtype)
-        noise = torch.randn(16, 16, device='cuda') * 0.3
-        b = torch.randn(6, device='cuda').to(dtype)
-        y = torch.empty(2, 6, 16, 16, device='cuda', dtype=dtype)
-        xs = (_lib.c_int32 * 4)(*x.shape)
-        ys = (_lib.c_int32 * 4)(*y.shape)
-        st = _lib.lib().p3d_fir_bias_act(_lib.ptr(x), _lib.ptr(f), None, _lib.ptr(noise), _lib.ptr(b), _lib.ptr(y),
-                                         _lib.DTYPE_CODE[dtype], xs, ys, 4, 4, 1, 1, 4.0, 3, 0.2, float(np.sqrt(2)), 256.0, 0,
-                                         _lib.stream_ptr())
-        _lib.check(st, 'p3d_fir_bias_act')
-        ref = upfirdn2d.upfirdn2d(x, f, padding=[1, 1, 1, 1], gain=4)
-        ref = ref.add_(noise)
-        ref = bias_act.bias_act(ref, b, act='lrelu', clamp=256)
-        assert rel_err(y.float().cpu().numpy(), ref.float().cpu().numpy()) < tol
-
-
 def test_filtered_lrelu_cuda_matches_oracle_and_reference():
     from pix2pix3d_b200.torch_utils.ops import filtered_lrelu
     g = load_golden('ops')

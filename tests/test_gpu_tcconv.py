@@ -388,7 +388,7 @@ def test_conv_gemm_phases_rejects_mismatched_phases():
     wk = _weights_kmajor(torch.randn(16, 64, 3, 3, device='cuda'))
     out = torch.zeros(1, 9, 9, 16, device='cuda', dtype=torch.float16)
     other = torch.zeros(1, 9, 9, 16, device='cuda', dtype=torch.float16)
-    arr = (tcconv.ConvArgs * 2)()
+    arr = (_lib.ConvArgs * 2)()
     arr[0] = tcconv._conv_args(x, wk, 16, tcconv.tconv_phase_taps(0, 0), (5, 5), out, out_map=(2, 0, 2, 0))
     arr[1] = tcconv._conv_args(x, wk, 16, tcconv.tconv_phase_taps(0, 1), (5, 4), other, out_map=(2, 0, 2, 1))
     assert _lib.lib().p3d_conv_gemm_phases(arr, 2, _lib.stream_ptr()) == -2

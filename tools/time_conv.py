@@ -17,7 +17,6 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 from pix2pix3d_b200 import _lib, configs, native  # noqa: E402
-from pix2pix3d_b200.tcconv import ConvArgs  # noqa: E402
 
 
 def ceil_div(a, b):
@@ -73,13 +72,13 @@ class _Recorder:
         st = self._h.p3d_conv_gemm(a, stream)
         if st == 0:
             src = a._obj
-            self.calls.append([ConvArgs.from_buffer_copy(src)])
+            self.calls.append([_lib.ConvArgs.from_buffer_copy(src)])
         return st
 
     def p3d_conv_gemm_phases(self, arr, n, stream):
         st = self._h.p3d_conv_gemm_phases(arr, n, stream)
         if st == 0:
-            self.calls.append([ConvArgs.from_buffer_copy(arr[k]) for k in range(n)])
+            self.calls.append([_lib.ConvArgs.from_buffer_copy(arr[k]) for k in range(n)])
         return st
 
 
